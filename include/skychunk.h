@@ -1,5 +1,5 @@
 /*
- * skychunk.h -- C ABI of the B200 chunk-processing stage (libskychunk.so).
+ * skychunk.h -- C ABI of the H100 chunk-processing stage (libskychunk.so).
  *
  * Drop-in boundary for the per-chunk hot path of Skyplane's gateway.  The reference has no FFI
  * (it is pure Python); these entry points replace, for one batch of chunks, the two calls

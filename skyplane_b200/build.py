@@ -1,4 +1,4 @@
-"""Builds libskychunk.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds libskychunk.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -14,11 +14,12 @@ SOURCES = [CSRC / "skychunk.cu"]
 
 
 def _deps():
-    return sorted(CSRC.glob("*.cu*")) + sorted((PKG.parent / "include").glob("*.h"))
+    # build.py itself: a change of NVCC_FLAGS (e.g. the target architecture) must rebuild the library
+    return sorted(CSRC.glob("*.cu*")) + sorted((PKG.parent / "include").glob("*.h")) + [Path(__file__).resolve()]
 
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC,-fvisibility=hidden",
     "-cudart", "static",

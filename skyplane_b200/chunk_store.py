@@ -2,7 +2,7 @@
 
 Layout the stage relies on:
   <chunk_dir>/<chunk_id>.chunk       the chunk's bytes (tmpfs in production, compute/server.py:341)
-  <chunk_dir>/<chunk_id>.chunk.lz4   ours: the LZ4 frame produced by / delivered to the B200 stage
+  <chunk_dir>/<chunk_id>.chunk.lz4   ours: the LZ4 frame produced by / delivered to the H100 stage
 Operators report state changes with ``log_chunk_state``; the records travel through ``chunk_status_queue`` to
 whoever plays the gateway API's role (gateway_daemon_api.py:89-155).
 """
@@ -100,7 +100,7 @@ class ChunkStore:
             worker_id=worker_id,
         )
         if metadata:
-            record.update(metadata)  # e.g. compressed_size_bytes / uncompressed_size_bytes from the B200 stage
+            record.update(metadata)  # e.g. compressed_size_bytes / uncompressed_size_bytes from the H100 stage
         self.chunk_status_queue.put(record)
 
     def log_chunk_states(self, chunk_reqs, new_status: ChunkState, worker_id: Optional[int] = None, operator_handle: Optional[str] = None,

@@ -1,4 +1,4 @@
-// lz4.cuh -- LZ4 block compressor for sm_100a: helpers shared by all formulations, and the CTA-per-block compressor
+// lz4.cuh -- LZ4 block compressor for sm_90a: helpers shared by all formulations, and the CTA-per-block compressor
 // (prober / parser warps over a shared-memory copy of the block) that sky_fused_kernel runs.
 //
 // Replaces, per 64 KiB block, what lz4.frame.compress(data) does inside
@@ -415,7 +415,7 @@ __device__ __noinline__ uint32_t flush_seqs(uint8_t *__restrict__ out, uint32_t 
 // that of the lane 3, 4 or 8 places below it takes that lane's slot as its candidate (three shuffles; periods 1, 2, 3, 4
 // and 8 -- runs, UTF-16, pixels, words, doubles -- which the table cannot know yet because a group looks the table up before
 // any of its slots is inserted).  Nothing here orders the lanes by hash: round 2's first formulation used match.any for
-// that, and at 58 cycles of the SM's one ADU pipe per instruction it was what bounded the kernel (profiles/README.md).
+// that, and the SM's one ADU pipe that executes it was what bounded the kernel.
 // `turn()` is called between the phases: it returns when the other prober has finished the previous batch's table phase.
 // Phase B -- the 8 table lookups and updates back to back: every lane reads its entry, then every lane max-es its own in
 // (position in the high half: of the lanes that share an index the highest one stays, exactly what inserting the slots in

@@ -1,10 +1,10 @@
-// lz4dec.cuh -- LZ4 frame decoder for the receiving gateway (SURVEY.md section 8f row 1), sm_100a.
+// lz4dec.cuh -- LZ4 frame decoder for the receiving gateway (SURVEY.md section 8f row 1), sm_90a.
 //
 // Replaces lz4.frame.decompress(to_write) at skyplane/gateway/operators/gateway_receiver.py:195-201.
 // Two device steps:
 //   frame_index : one lane per chunk checks the frame header (magic, FLG, BD, content size, header checksum)
 //                 and walks the block headers, producing a block table (offset, size word) per chunk;
-//   block decode: one warp per 64 KiB block.  Frames whose blocks are independent (what the B200 sender
+//   block decode: one warp per 64 KiB block.  Frames whose blocks are independent (what the H100 sender
 //                 emits) decode fully in parallel; linked-block frames (what the reference's CPU sender emits)
 //                 decode block j after block j-1 of the same chunk (matches may reach into earlier output).
 // Every read and write is bounds-checked: a malformed frame yields an error status, never an out-of-range access.

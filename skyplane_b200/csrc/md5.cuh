@@ -1,4 +1,4 @@
-// md5.cuh -- RFC 1321 MD5, one digest stream per lane, for sm_100a.
+// md5.cuh -- RFC 1321 MD5, one digest stream per lane, for sm_90a.
 //
 // Replaces hashlib.md5().update()/digest() at skyplane/obj_store/s3_interface.py:181-192.
 // One chunk is ONE serial chain (the digest must equal hashlib.md5(whole chunk)), so a warp

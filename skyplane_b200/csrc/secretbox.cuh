@@ -1,4 +1,4 @@
-// secretbox.cuh -- XSalsa20-Poly1305 (NaCl crypto_secretbox) on sm_100a, behind the LZ4 frame.
+// secretbox.cuh -- XSalsa20-Poly1305 (NaCl crypto_secretbox) on sm_90a, behind the LZ4 frame.
 //
 // Replaces, per chunk, the CPU call the sender makes when end-to-end encryption is on
 //     data = nacl.secret.SecretBox(key).encrypt(data)            skyplane/gateway/operators/gateway_operator.py:362-364

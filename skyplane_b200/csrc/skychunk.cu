@@ -1,9 +1,9 @@
-// skychunk.cu -- fused LZ4-frame + MD5 chunk stage for B200 (sm_100a) and its C ABI (include/skychunk.h).
+// skychunk.cu -- fused LZ4-frame + MD5 chunk stage for H100 (sm_90a) and its C ABI (include/skychunk.h).
 //
 // One persistent kernel per batch (sky_fused_kernel), two CTAs per SM, 14 warps per CTA, one role per CTA at a time:
 //   * digest CTAs : the first few CTAs carry the MD5 groups -- 32 chunks per warp, lane = chunk (md5.cuh), one MD5 warp
 //                   per CTA while the groups are few.  An MD5 chain is latency bound (3 dependent ALU ops per step, one
-//                   64-byte block per 1042 cycles) and keeps its scheduler's issue port busy; when a CTA's groups are done
+//                   64-byte block per ~1044 cycles) and keeps its scheduler's issue port busy; when a CTA's groups are done
 //                   it joins the compressors.
 //   * compressor CTAs : one 64 KiB block at a time, claimed from a global atomic counter in row-major order (block row j of
 //                   every chunk, then row j+1 ...): bulk-load the block into shared memory, warps 0-1 probe, warps 2-13
@@ -359,7 +359,7 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) 
                 bool got = true;
                 // (mbarrier.try_wait's hardware suspend ends at every barrier event in the CTA, a few dozen ns apart here, so the
                 // waiting loops are a quarter of the instructions issued -- but replacing them with timed sleeps gained
-                // nothing (r2_29: 115.9 vs 116.3 GB/s): the issue slots they take are not the ones the parsers lack.)
+                // nothing measurable: the issue slots they take are not the ones the parsers lack.)
                 unsigned ns = 32;
                 while (!(kWaitNs ? mbar_test_wait(&ctl->full[si], ph) : mbar_try_wait_hint(&ctl->full[si], ph, 1000u))) {
                     if (atomicAdd(const_cast<uint32_t *>(&ctl->block_end_seq), 0u) <= my_seq) {  // no such segment in this block: keep the claim
@@ -890,7 +890,7 @@ int sky_ctx_create(int device, uint64_t max_batch_bytes, uint32_t max_chunks, ui
     e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (e != cudaSuccess) {
-        ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (built for sm_100a only)";
+        ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (this build carries sm_90a code only)";
         return fail(SKY_E_CUDA);
     }
     const uint32_t ns = n_slots ? n_slots : 1;
@@ -1048,10 +1048,9 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
     p.n_chunks = n;
     p.n_groups = ng;
     const uint32_t grid = (uint32_t)ctx->sm_count * kCtasPerSm;
-    // digest CTAs: 4 groups (one per SM sub-partition) each; with few groups spread them one per CTA first.  (Tried in
-    // r2_30 / r2_31: whole digest SMs -- 4 or 8 MD5 warps on a few SMs, nothing else there -- so that fewer block buffers
-    // sit idle.  With 8 or 16 MiB chunks the MD5 warps then ran at half their chain rate (0.061 GB/s per chunk; with 1 MiB
-    // chunks at the full 0.118), so the spread-out arrangement stays.)
+    // digest CTAs: 4 groups (one per SM sub-partition) each; with few groups spread them one per CTA first.  (Whole digest
+    // SMs -- 4 or 8 MD5 warps on a few SMs, nothing else there -- would leave fewer block buffers idle, but with 8 or 16 MiB
+    // chunks such packed MD5 warps ran at about half their chain rate, so the spread-out arrangement stays.)
     {
         // MD5 warps per digest CTA while the groups are few: 1 = one warp in each of up to sm_count / 4 CTAs (default);
         // SKYCHUNK_MD5_WARPS=2 packs two per CTA so that half as many block buffers sit idle in the fused kernel (tuning knob)

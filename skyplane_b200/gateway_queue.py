@@ -3,7 +3,7 @@
 * ``GatewayQueue``    -- one bounded multiprocessing queue shared by the workers of the consuming operator.
 * ``GatewayANDQueue`` -- fan-out: every registered consumer handle gets its own ``GatewayQueue`` and sees every item.
 
-``get_batch_nowait`` is ours: the B200 operator drains many requests per kernel launch.
+``get_batch_nowait`` is ours: the H100 operator drains many requests per kernel launch.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""The reference's three file-only operators, so complete local pipelines can be wired around the B200 stage
+"""The reference's three file-only operators, so complete local pipelines can be wired around the H100 stage
 (``gen_data -> compress_hash -> ... -> decompress_verify -> write_local``) without any cloud or socket code.
 
 Behavioural mirrors of skyplane/gateway/operators/gateway_operator.py:

@@ -1,4 +1,4 @@
-"""Gateway operator plugin surface + the B200 compress/hash operator.
+"""Gateway operator plugin surface + the H100 compress/hash operator.
 
 ``GatewayOperator`` keeps the reference's contract (skyplane/gateway/operators/gateway_operator.py:32-122):
 same constructor arguments, ``start_workers`` forks ``n_processes`` workers running
@@ -111,7 +111,7 @@ class GatewayOperator(ABC):
 
 
 class GatewayCompressHash(GatewayOperator):
-    """B200 stage: LZ4 frame + MD5 per chunk, batched per kernel launch."""
+    """H100 stage: LZ4 frame + MD5 per chunk, batched per kernel launch."""
 
     def __init__(
         self,
@@ -146,7 +146,7 @@ class GatewayCompressHash(GatewayOperator):
         self.sink = sink
         # batches in flight per worker: a batch of 8 MiB chunks spends >= 70 ms on the GPU whatever its size (one serial MD5
         # chain per chunk), so throughput = chunks in flight / 70 ms -- keep several batches going (one slot is being read
-        # into, the others are on the GPU; measured 18.8 / 26.5 / 27.2 / 26.2 GB/s with 3 / 4 / 5 / 6 slots of 128 chunks)
+        # into, the others are on the GPU)
         self.n_slots = max(2, n_slots)
         self._sock = None
         self.max_batch_chunks = max_batch_chunks

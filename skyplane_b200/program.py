@@ -8,7 +8,7 @@ and the daemon consumes in ``create_gateway_operators`` (skyplane/gateway/gatewa
 Wiring rules kept from the reference: a node's handle is ``<op_type>_<handle>``; an operator whose first child
 is ``mux_and`` feeds a ``GatewayANDQueue`` (every grandchild sees every chunk), ``mux_or`` children share the
 private queue their ``mux_and`` parent gave them, operators without children are terminal, an unknown ``op_type``
-raises ``ValueError``.  Built in: the B200 stage's op types (``compress_hash`` between ``read_object_store`` and
+raises ``ValueError``.  Built in: the H100 stage's op types (``compress_hash`` between ``read_object_store`` and
 ``send`` on the source gateway, ``decompress_verify`` before ``write_object_store`` on the destination gateway) and the
 reference's three file-only operators (``receive``, ``gen_data``, ``write_local``); the daemon's cloud / socket
 operators (object store, sender) are supplied by the caller through ``factories``.

@@ -1,4 +1,4 @@
-"""ChunkStage: the host side of the B200 compress+hash stage (pinned staging + libskychunk).
+"""ChunkStage: the host side of the H100 compress+hash stage (pinned staging + libskychunk).
 
 This is what replaces, for a batch of chunks, the reference's two per-chunk CPU calls
 (``lz4.frame.compress`` at skyplane/gateway/operators/gateway_operator.py:359 and the

@@ -13,7 +13,7 @@ GOLDEN = Path(__file__).resolve().parent / "golden"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100 box)")
 
 
 def _has_gpu() -> bool:

@@ -1,4 +1,4 @@
-"""Generates the committed golden fixtures (run in the build container, where /root/reference exists).
+"""Generates the committed golden fixtures (needs a checkout of the reference, skyplane @ 4602d9c).
 
   wire_headers.json  WireProtocolHeader.to_bytes() produced by the REFERENCE's own skyplane/chunk.py
                      (imported by file path -- it is stdlib-only) for a handful of field values,
@@ -8,7 +8,7 @@
   lz4_frames.json    small inputs and the exact frames liblz4 1.9.4 LZ4F_compressFrame emits for them with
                      python-lz4's default preferences (what lz4.frame.compress(data) returns,
                      gateway_operator.py:359), via oracle/reflib.py.
-Usage: python tests/golden/make_golden.py
+Usage: python tests/golden/make_golden.py <path of the skyplane checkout>
 """
 import hashlib
 import importlib.util
@@ -26,7 +26,7 @@ import oracle.reflib as ref  # noqa: E402
 
 
 def load_reference_chunk():
-    spec = importlib.util.spec_from_file_location("ref_chunk", "/root/reference/skyplane/chunk.py")
+    spec = importlib.util.spec_from_file_location("ref_chunk", Path(sys.argv[1]) / "skyplane" / "chunk.py")
     mod = importlib.util.module_from_spec(spec)
     sys.modules["ref_chunk"] = mod
     spec.loader.exec_module(mod)

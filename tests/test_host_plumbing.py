@@ -205,9 +205,9 @@ def test_frame_bound_and_strerror_without_gpu():
     assert b"no CUDA device" in native.lib().sky_strerror(native.SKY_E_NOGPU)
 
 
-def test_library_carries_sm100a_code():
+def test_library_carries_sm90a_code():
     out = subprocess.run(["cuobjdump", "-lelf", str(native.LIB_PATH)], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 @pytest.mark.skipif(native.device_count() > 0, reason="only meaningful on a box without a GPU")

@@ -1,10 +1,10 @@
-// md5_chain_bench.cu -- measures the dependent-chain latency of one MD5 block per lane on sm_100a
+// md5_chain_bench.cu -- measures the dependent-chain latency of one MD5 block per lane on sm_90a
 // for several instruction selections of the on-chain add.  Not product code: a measurement tool whose
 // result picks the formulation used in skyplane_b200/csrc/md5.cuh.
 //   V0: plain C (ptxas picks IMAD.IADD for the on-chain add: alu -> fma -> alu)
 //   V1: on-chain add forced onto the ALU pipe by consuming its carry (IADD3 with carry-out)
 //   V2: 3-input on-chain add (a, m+K, f) kept separate via carry trick on the inner add
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o md5_chain_bench tools/md5_chain_bench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bin/md5_chain_bench tools/md5_chain_bench.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
