@@ -35,7 +35,7 @@ extern "C" {
 #define SKY_API
 #endif
 
-#define SKY_ABI_VERSION 2
+#define SKY_ABI_VERSION 3
 
 /* error codes */
 #define SKY_OK 0
@@ -52,13 +52,7 @@ extern "C" {
  * gateway_operator.py:358): the chunk is digested and passes through uncompressed. */
 #define SKY_F_LZ4 1u
 #define SKY_F_MD5 2u
-/* accepted and ignored since ABI 2 (round 1 kept an SM sub-partition free for each MD5 warp; digest groups now run in
- * CTAs of their own) */
-#define SKY_F_MD5_EXCLUSIVE 4u
-/* do not pace LZ4 work to the MD5 lanes' progress (pacing lets the lanes read the input from L2; sky_submit always
- * runs unpaced so that the kernels of different slots overlap) */
-#define SKY_F_NO_PACING 8u
-/* end-to-end encryption behind the frame (sky_submit_flags / sky_decode_flags): every payload becomes PyNaCl's
+/* end-to-end encryption behind the frame (sky_submit / sky_decode): every payload becomes PyNaCl's
  * SecretBox.encrypt() message  nonce(24) | tag(16) | ciphertext  (XSalsa20-Poly1305), as GatewaySender does with
  * e2ee_key_bytes (gateway_operator.py:183-186, :362-364) and the receiver undoes (gateway_receiver.py:191-193). */
 #define SKY_F_E2EE 16u
@@ -97,18 +91,16 @@ SKY_API int sky_pinned_free(void *p);
  *   per-chunk sizes and digests back.  src[i]/src_len[i] = chunk bytes; dst[i]/dst_cap[i] = where
  *   the frame goes (dst_cap[i] >= sky_frame_bound(src_len[i])).  All host buffers must stay valid
  *   until sky_wait returns.  Pinned buffers make the copies truly asynchronous.
+ *   flags: SKY_F_* (0 = LZ4 + MD5, nonces may be NULL).  SKY_F_MD5 alone: digests only (dst / dst_cap may be NULL,
+ *   out_len comes back 0: the caller forwards its own input bytes, is_compressed = False).  | SKY_F_E2EE: what comes
+ *   back in dst[i] is the sealed box of the frame (or of the raw chunk when SKY_F_LZ4 is off), out_len[i] = its length
+ *   = payload + SKY_BOX_OVERHEAD, dst_cap[i] >= sky_box_bound(src_len[i]); nonces = 24 bytes per chunk chosen by the
+ *   caller (nacl.utils.random(24)).  The key is the ctx's (sky_set_e2ee_key; key32 = NULL switches E2EE off).
  * sky_wait: blocks until the batch is done, copies each frame device->host (exact length), and
  *   fills out_len[n], md5[16*n].  kernel_ms (optional) = device time of the fused kernel. */
 SKY_API int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t *src_len, void *const *dst,
-               const uint64_t *dst_cap, uint64_t *ticket);
+               const uint64_t *dst_cap, uint32_t flags, const uint8_t *nonces, uint64_t *ticket);
 SKY_API int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, float *kernel_ms);
-/* sky_submit with stage flags.  flags = SKY_F_MD5: digests only (dst / dst_cap may be NULL, out_len comes back 0: the
- *   caller forwards its own input bytes, is_compressed = False).  | SKY_F_E2EE: what comes back in dst[i] is the sealed
- *   box of the frame (or of the raw chunk when SKY_F_LZ4 is off), out_len[i] = its length = payload + SKY_BOX_OVERHEAD,
- *   dst_cap[i] >= sky_box_bound(src_len[i]); nonces = 24 bytes per chunk chosen by the caller (nacl.utils.random(24)).
- *   The key is the ctx's (sky_set_e2ee_key; key32 = NULL switches E2EE off). */
-SKY_API int sky_submit_flags(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t *src_len, void *const *dst,
-                     const uint64_t *dst_cap, uint32_t flags, const uint8_t *nonces, uint64_t *ticket);
 SKY_API int sky_set_e2ee_key(sky_ctx *ctx, const uint8_t *key32);
 SKY_API uint64_t sky_box_bound(uint64_t n); /* sky_frame_bound(n) + SKY_BOX_OVERHEAD */
 
@@ -130,7 +122,9 @@ SKY_API int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, cons
  * error status, never a crash); md5[16*i..] = MD5 of the decoded bytes.
  * sky_decode_device: frames and output already in HBM (out_off multiples of 16; each frame region must be readable
  * up to the next multiple of 4 bytes, each output region writable up to the next multiple of 16).  sky_decode: host
- * buffers, synchronous, through slot 0's slabs (needs n_slots >= 1). */
+ * buffers, synchronous, through slot 0's slabs (needs n_slots >= 1); flags = 0, or SKY_F_E2EE: the payloads are sealed
+ * boxes, whose tags are checked and which are opened on the device before the frames are decoded (status SKY_D_AUTH for
+ * a forged / truncated box, whose bytes are never returned). */
 #define SKY_D_OK 0
 #define SKY_D_BAD_HEADER (-1)
 #define SKY_D_CORRUPT (-2)
@@ -143,11 +137,7 @@ SKY_API int sky_decode_device(sky_ctx *ctx, uint32_t n, const void *d_frames, co
                       void *d_out, const uint64_t *out_off, const uint64_t *raw_len, void *stream, int32_t *status, uint8_t *md5,
                       float *kernel_ms);
 SKY_API int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64_t *frame_len, void *const *dst,
-               const uint64_t *raw_len, int32_t *status, uint8_t *md5, float *kernel_ms);
-/* sky_decode with flags: SKY_F_E2EE = the payloads are sealed boxes; tags are checked and the boxes opened on the device
- * before the frames are decoded (status SKY_D_AUTH for a forged / truncated box, whose bytes are never returned). */
-SKY_API int sky_decode_flags(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64_t *frame_len, void *const *dst,
-                     const uint64_t *raw_len, uint32_t flags, int32_t *status, uint8_t *md5, float *kernel_ms);
+               const uint64_t *raw_len, uint32_t flags, int32_t *status, uint8_t *md5, float *kernel_ms);
 
 /* Device-memory helpers so a host without torch can drive the device path. */
 SKY_API int sky_device_alloc(sky_ctx *ctx, uint64_t bytes, void **dptr);

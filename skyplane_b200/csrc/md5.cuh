@@ -134,8 +134,6 @@ __device__ __forceinline__ void cp_async_wait() {
 // Digest of one chunk per lane.  `ring` = this warp's 8 KiB shared-memory area (2048 x uint32),
 // `src` 16-byte aligned (or len == 0), `active` false for lanes without a chunk.
 // Writes 16 digest bytes to `out` for active lanes.
-// `progress` (may be null): lane 0 publishes how many 64 KiB rows the warp has consumed, so LZ4 warps can
-// fetch a row just ahead of the MD5 lanes and the lanes then hit L2 instead of HBM.
 // `gate(row, wants)`: called (warp-converged) before the first byte of 64 KiB row `row` is fetched; `wants` tells
 // whether this lane has data in that row.  The receiver side uses it to wait until the row has been decoded.
 struct Md5NoGate {
@@ -144,7 +142,7 @@ struct Md5NoGate {
 
 template <class Gate = Md5NoGate>
 __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uint64_t len, bool active, uint8_t *out,
-                                         unsigned lane, volatile uint32_t *progress, Gate gate = Gate()) {
+                                         unsigned lane, Gate gate = Gate()) {
     constexpr int kSlots = SKY_MD5_SLOTS;  // ring depth (blocks, power of two); prefetch distance = kSlots - 1
     constexpr bool kGated = !std::is_same<Gate, Md5NoGate>::value;
     const uint64_t nfull = active ? (len >> 6) : 0;
@@ -208,12 +206,8 @@ __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uin
             for (uint64_t i = base; i < iend; i++) SKY_MD5_LOOP_BODY(i)
         }
     } else {
-        // Sender side: one flat loop (measured 1.027x faster per block than the nested form); lane 0 publishes the
-        // rows consumed so LZ4 warps can stay just ahead of the digest lanes.
-        for (uint64_t i = 0; i < wmax; i++) {
-            SKY_MD5_LOOP_BODY(i)
-            if (progress && lane == 0 && ((i + 1) & 1023) == 0) *progress = (uint32_t)((i + 1) >> 10) + 1u;  // 1 + 64 KiB rows done
-        }
+        // Sender side: one flat loop (measured 1.027x faster per block than the nested form).
+        for (uint64_t i = 0; i < wmax; i++) SKY_MD5_LOOP_BODY(i)
     }
 #undef SKY_MD5_LOOP_BODY
     cp_async_wait<0>();

@@ -16,8 +16,7 @@
 // writes its bytes to the final place exactly once (stored blocks straight from the input).  The last block's CTA writes
 // the EndMark and the frame length.
 //
-// HBM-read sharing: when MD5 is the slower stage, LZ4 work for block row j is released only when the MD5 lanes have entered
-// that row (per-group progress word), so a row is pulled from HBM once and the lanes find it in L2.
+// The two roles never wait on each other: digest lanes and compressors each read their own input from HBM.
 //
 // Host side: sky_ctx owns a stream, pinned + device metadata arrays, and (optionally) per-slot input /
 // output slabs for the host-buffer path (H2D -> kernel -> D2H on one stream per slot).
@@ -53,14 +52,6 @@ constexpr int kThreads = kWarps * 32;
 #ifndef SKY_RING_EXTRA
 #define SKY_RING_EXTRA 2
 #endif
-#ifndef SKY_WAIT_NS
-#define SKY_WAIT_NS 0
-#endif
-#ifndef SKY_PACE_LEAD
-#define SKY_PACE_LEAD 0
-#endif
-constexpr uint32_t kWaitNs = SKY_WAIT_NS;       // 0: a waiting parser is parked by mbarrier.try_wait (measured best); else it sleeps, doubling up to this many ns
-constexpr uint32_t kPaceLead = SKY_PACE_LEAD;   // rows the compressor may run ahead of a chunk's MD5 lanes beyond the one they are in
 constexpr int kRing = kParsers + SKY_RING_EXTRA;       // segment slots between the prober and the parsers
 constexpr int kMd5WarpsPerCta = 4;        // digest CTAs run 4 MD5 groups (one per SM sub-partition), see sky_fused_kernel
 constexpr uint32_t kRingBytes = SKY_MD5_SLOTS * 2048;  // MD5 staging ring: slots x 64 B x 32 lanes
@@ -105,14 +96,12 @@ struct ChunkDesc {
     uint8_t *dst;        // 16-byte aligned
     uint64_t len;
     uint32_t nblk;
-    uint32_t group;  // MD5 group (warp) that digests this chunk
 };
 
 struct Params {
     const ChunkDesc *chunks;
     const uint32_t *md5_order;  // chunk indices, longest first, padded with 0xffffffff to 32*n_groups
     uint64_t *chain;            // per chunk OFF word: (next block index << 40) | frame offset of that block
-    uint32_t *md5_progress;     // per MD5 group: 0 = not started, else 1 + 64 KiB rows consumed (0xffffffff = done)
     uint64_t *out_len;          // per chunk frame length
     uint8_t *md5_out;           // 16 bytes per chunk
     uint32_t *counters;         // [0] = LZ4 work counter
@@ -145,15 +134,9 @@ template <int kId>
 __device__ __forceinline__ void bar_arrive() { asm volatile("bar.arrive %0, 64;" ::"n"(kId) : "memory"); }
 template <int kId>
 __device__ __forceinline__ void bar_wait() { asm volatile("bar.sync %0, 64;" ::"n"(kId) : "memory"); }
-__device__ __forceinline__ uint32_t ld_relaxed32(const uint32_t *p) {
-    uint32_t v;
-    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
 
-// Prober lane 0: claim the next block that has LZ4 work (empty chunks are finished on the spot), wait until the chunk's
-// MD5 lanes are close (so the block is read from HBM once), and describe it to the CTA.
-__device__ __forceinline__ void claim_block(const Params &p, BlockDesc *d, bool pace) {
+// Prober lane 0: claim the next block that has LZ4 work (empty chunks are finished on the spot) and describe it to the CTA.
+__device__ __forceinline__ void claim_block(const Params &p, BlockDesc *d) {
     const uint32_t total = p.rows * p.n_chunks;
     for (;;) {
         const uint32_t w = atomicAdd(p.counters, 1u);
@@ -172,22 +155,6 @@ __device__ __forceinline__ void claim_block(const Params &p, BlockDesc *d, bool 
             continue;
         }
         if (j >= cd.nblk) continue;
-        if (pace) {
-            // stay at most one 64 KiB row ahead of the MD5 lanes of this chunk (only while they are running); the last
-            // rows may run up to kTailLead rows ahead so the compressor's own latency for the final row overlaps the
-            // digest's last rows instead of trailing them
-            const uint32_t *pw = p.md5_progress + cd.group;
-            constexpr uint32_t kTailLead = 8;
-            const uint32_t lead = (cd.nblk - j <= kTailLead) ? kTailLead : 0;
-            unsigned ns = 64;
-            for (;;) {
-                const uint32_t pr = ld_relaxed32(pw);
-                // pr: 0 = digest not started, 0xffffffff = finished, else 1 + rows consumed (64-bit compare: no wrap)
-                if (pr == 0 || (uint64_t)j + 1 <= (uint64_t)pr + lead + kPaceLead) break;
-                __nanosleep(ns);
-                if (ns < 4096) ns <<= 1;
-            }
-        }
         const uint64_t boff = (uint64_t)j * kBlock;
         d->src = cd.src + boff;
         d->dst = cd.dst;
@@ -244,11 +211,8 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) 
                     src = p.chunks[c].src;
                     len = p.chunks[c].len;
                 }
-                volatile uint32_t *prog = p.md5_progress + g;
-                if (lane == 0) *prog = 1u;  // started, 0 rows consumed
                 md5_warp(reinterpret_cast<uint32_t *>(in + warp * kRingBytes), src, len, active, p.md5_out + (size_t)(active ? c : 0) * 16,
-                         lane, prog);
-                if (lane == 0) *prog = 0xffffffffu;
+                         lane);
                 __syncwarp();
             }
         }
@@ -257,7 +221,6 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) 
     }
     if (!do_lz4) return;
 
-    const bool pace = do_md5 && !(p.flags & SKY_F_NO_PACING);
     uint8_t *scratch = p.scratch + (size_t)blockIdx.x * kScratchBytes;
     uint32_t gseq = 0;        // probers: sequence number of the next segment they publish (runs across blocks)
     uint32_t batches_done = 0;  // prober 0: nothing to wait for before the kernel's very first batch
@@ -267,7 +230,7 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) 
     for (uint32_t it = 0;; it++) {
         BlockDesc *dsc = &ctl->desc[it & 1];
         if (warp == 0 && lane == 0) {
-            claim_block(p, dsc, pace);
+            claim_block(p, dsc);
             ctl->block_end_seq = 0xffffffffu;
             ctl->nseg = 0;
         }
@@ -360,15 +323,10 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) 
                 // (mbarrier.try_wait's hardware suspend ends at every barrier event in the CTA, a few dozen ns apart here, so the
                 // waiting loops are a quarter of the instructions issued -- but replacing them with timed sleeps gained
                 // nothing measurable: the issue slots they take are not the ones the parsers lack.)
-                unsigned ns = 32;
-                while (!(kWaitNs ? mbar_test_wait(&ctl->full[si], ph) : mbar_try_wait_hint(&ctl->full[si], ph, 1000u))) {
+                while (!mbar_try_wait_hint(&ctl->full[si], ph, 1000u)) {
                     if (atomicAdd(const_cast<uint32_t *>(&ctl->block_end_seq), 0u) <= my_seq) {  // no such segment in this block: keep the claim
                         got = mbar_try_wait(&ctl->full[si], ph);
                         break;
-                    }
-                    if (kWaitNs) {
-                        __nanosleep(ns);
-                        if (ns < kWaitNs) ns <<= 1;
                     }
                 }
                 if (!got) break;
@@ -578,7 +536,7 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
                 gate.flags = p.blk_done + p.chunks[c].blk_base;
             }
             md5_warp(reinterpret_cast<uint32_t *>(smem + warp * kRingBytes), src, len, active, p.md5_out + (size_t)(active ? c : 0) * 16,
-                     lane, nullptr, gate);
+                     lane, gate);
             __syncwarp();
         }
     }
@@ -686,7 +644,7 @@ struct Slot {
     ChunkDesc *h_desc = nullptr, *d_desc = nullptr;
     uint32_t *h_order = nullptr, *d_order = nullptr;
     uint64_t *h_chain = nullptr, *d_chain = nullptr;
-    uint32_t *d_freed = nullptr, *d_progress = nullptr;
+    uint32_t *d_freed = nullptr;
     // results live in MAPPED pinned host memory: the kernel stores sizes / digests straight over PCIe, so no small
     // device->host copies sit in a copy-engine queue behind multi-GiB frame copies
     uint64_t *h_outlen = nullptr, *d_outlen = nullptr;  // same allocation, host / device view
@@ -831,7 +789,6 @@ static int alloc_meta(sky_ctx *ctx, Slot &s, uint32_t max_chunks) {
     CK(ctx, cudaMallocHost(&s.h_dstatus, nc * sizeof(int32_t)));
     CK(ctx, cudaMalloc(&s.d_dstatus, nc * sizeof(int32_t)));
     CK(ctx, cudaMalloc(&s.d_freed, nc * sizeof(uint32_t)));
-    CK(ctx, cudaMalloc(&s.d_progress, (ng / 32 + 1) * sizeof(uint32_t)));
     CK(ctx, cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
     CK(ctx, cudaEventCreate(&s.ev_k0));
     CK(ctx, cudaEventCreate(&s.ev_k1));
@@ -846,7 +803,7 @@ static void free_slot(Slot &s) {
     if (s.stream) cudaStreamSynchronize(s.stream);
     cudaFreeHost(s.h_desc); cudaFreeHost(s.h_order); cudaFreeHost(s.h_chain); cudaFreeHost(s.h_outlen); cudaFreeHost(s.h_md5);
     cudaFree(s.d_desc); cudaFree(s.d_order); cudaFree(s.d_chain); cudaFree(s.d_counters);
-    cudaFreeHost(s.h_dchunks); cudaFree(s.d_dchunks); cudaFree(s.d_dblocks); cudaFree(s.d_blkdone); cudaFreeHost(s.h_dstatus); cudaFree(s.d_dstatus); cudaFree(s.d_freed); cudaFree(s.d_progress);
+    cudaFreeHost(s.h_dchunks); cudaFree(s.d_dchunks); cudaFree(s.d_dblocks); cudaFree(s.d_blkdone); cudaFreeHost(s.h_dstatus); cudaFree(s.d_dstatus); cudaFree(s.d_freed);
     cudaFree(s.d_in); cudaFree(s.d_out); cudaFree(s.d_scratch);
     cudaFree(s.d_box); cudaFree(s.d_bchunks); cudaFree(s.d_blkbase); cudaFree(s.d_sub); cudaFree(s.d_nonce); cudaFreeHost(s.h_nonce);
     cudaFree(s.d_boxmeta); cudaFreeHost(s.h_boxmeta); cudaFree(s.d_bstatus); cudaFreeHost(s.h_bstatus);
@@ -997,6 +954,16 @@ static int launch_seal(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, uint8
     return SKY_OK;
 }
 
+// MD5 lane assignment (sender and receiver): chunk indices longest first, so a warp's 32 lanes carry similar lengths,
+// padded with 0xffffffff to whole groups of 32.  Returns the number of groups.
+static uint32_t fill_md5_order(uint32_t *order, uint32_t n, const uint64_t *len) {
+    const uint32_t ng = (n + 31) / 32;
+    std::iota(order, order + n, 0u);
+    std::stable_sort(order, order + n, [&](uint32_t a, uint32_t b) { return len[a] > len[b]; });
+    std::fill(order + n, order + ng * 32, 0xffffffffu);
+    return ng;
+}
+
 // Fills the slot's metadata for a batch and enqueues: meta H2D, counter reset, fused kernel, results D2H.
 // `meta_st`: stream the three small metadata copies ride on (the H2D stream on the host path, so they are
 // never queued behind another batch's frame copies); `st`: the stream the kernel runs on.
@@ -1012,17 +979,11 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
         const uint64_t nb = (src_len[i] + kBlock - 1) / kBlock;
         if (nb >= (1ull << 24)) return SKY_E_CAPACITY;
         d.nblk = (uint32_t)nb;
-        d.group = 0;
         rows = std::max(rows, d.nblk);
         s.h_chain[i] = 15;  // block 0 starts right after the 15-byte frame header
     }
     if ((uint64_t)rows * n >= 0xffffffffull) return SKY_E_CAPACITY;
-    // MD5 lane assignment: longest chunks first so a warp's 32 lanes carry similar lengths
-    const uint32_t ng = (n + 31) / 32;
-    std::iota(s.h_order, s.h_order + n, 0u);
-    std::stable_sort(s.h_order, s.h_order + n, [&](uint32_t a, uint32_t b) { return src_len[a] > src_len[b]; });
-    for (uint32_t i = n; i < ng * 32; i++) s.h_order[i] = 0xffffffffu;
-    for (uint32_t i = 0; i < n; i++) s.h_desc[s.h_order[i]].group = i / 32;
+    const uint32_t ng = fill_md5_order(s.h_order, n, src_len);
 
     CK(ctx, cudaMemcpyAsync(s.d_desc, s.h_desc, n * sizeof(ChunkDesc), cudaMemcpyHostToDevice, meta_st));
     CK(ctx, cudaMemcpyAsync(s.d_order, s.h_order, ng * 32 * sizeof(uint32_t), cudaMemcpyHostToDevice, meta_st));
@@ -1032,7 +993,6 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
         CK(ctx, cudaStreamWaitEvent(st, s.ev_h2d, 0));
     }
     CK(ctx, cudaMemsetAsync(s.d_counters, 0, 64, st));
-    CK(ctx, cudaMemsetAsync(s.d_progress, 0, (ng + 1) * sizeof(uint32_t), st));
     memset(s.h_outlen, 0, n * sizeof(uint64_t));  // host-side clear (mapped memory; the slot is idle here)
     memset(s.h_md5, 0, (size_t)n * 16);
 
@@ -1040,7 +1000,6 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
     p.chunks = s.d_desc;
     p.md5_order = s.d_order;
     p.chain = s.d_chain;
-    p.md5_progress = s.d_progress;
     p.out_len = s.d_outlen;
     p.md5_out = s.d_md5;
     p.counters = s.d_counters;
@@ -1051,17 +1010,8 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
     // digest CTAs: 4 groups (one per SM sub-partition) each; with few groups spread them one per CTA first.  (Whole digest
     // SMs -- 4 or 8 MD5 warps on a few SMs, nothing else there -- would leave fewer block buffers idle, but with 8 or 16 MiB
     // chunks such packed MD5 warps ran at about half their chain rate, so the spread-out arrangement stays.)
-    {
-        // MD5 warps per digest CTA while the groups are few: 1 = one warp in each of up to sm_count / 4 CTAs (default);
-        // SKYCHUNK_MD5_WARPS=2 packs two per CTA so that half as many block buffers sit idle in the fused kernel (tuning knob)
-        static const uint32_t md5_warps = [] {
-            const char *e = getenv("SKYCHUNK_MD5_WARPS");
-            const int v = e ? atoi(e) : 1;
-            return (uint32_t)(v >= 1 && v <= kMd5WarpsPerCta ? v : 1);
-        }();
-        p.n_md5_ctas = (flags & SKY_F_MD5) ? std::min(grid, std::max((ng + kMd5WarpsPerCta - 1) / kMd5WarpsPerCta,
-                                                                     std::min((ng + md5_warps - 1) / md5_warps, (uint32_t)ctx->sm_count / 4))) : 0;
-    }
+    p.n_md5_ctas = (flags & SKY_F_MD5) ? std::min(grid, std::max((ng + kMd5WarpsPerCta - 1) / kMd5WarpsPerCta,
+                                                                 std::min(ng, (uint32_t)ctx->sm_count / 4))) : 0;
     p.rows = rows;
     p.flags = flags;
     CK(ctx, cudaEventRecord(s.ev_k0, st));
@@ -1109,7 +1059,7 @@ int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64
                        void *d_dst, const uint64_t *dst_off, const uint64_t *dst_cap, uint32_t flags, void *stream,
                        uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
     if (!ctx || n == 0 || !src_off || !src_len || !dst_off || !dst_cap || !d_dst) return SKY_E_INVALID;
-    if (flags & SKY_F_E2EE) return SKY_E_INVALID;  // boxes are a host-path feature (sky_submit_flags)
+    if (flags & SKY_F_E2EE) return SKY_E_INVALID;  // boxes are a host-path feature (sky_submit)
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
     if ((reinterpret_cast<uintptr_t>(d_src) & 15) || (reinterpret_cast<uintptr_t>(d_dst) & 15)) return SKY_E_INVALID;
     for (uint32_t i = 0; i < n; i++) {
@@ -1131,12 +1081,7 @@ int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64
 }
 
 int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t *src_len, void *const *dst,
-               const uint64_t *dst_cap, uint64_t *ticket) {
-    return sky_submit_flags(ctx, n, src, src_len, dst, dst_cap, 0, nullptr, ticket);
-}
-
-int sky_submit_flags(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t *src_len, void *const *dst,
-                     const uint64_t *dst_cap, uint32_t flags, const uint8_t *nonces, uint64_t *ticket) {
+               const uint64_t *dst_cap, uint32_t flags, const uint8_t *nonces, uint64_t *ticket) {
     if (!ctx || n == 0 || !src || !src_len || !ticket) return SKY_E_INVALID;
     if ((flags & (SKY_F_LZ4 | SKY_F_MD5)) == 0) flags |= SKY_F_LZ4 | SKY_F_MD5;
     const bool e2ee = (flags & SKY_F_E2EE) != 0, frames = (flags & SKY_F_LZ4) != 0;
@@ -1168,16 +1113,12 @@ int sky_submit_flags(sky_ctx *ctx, uint32_t n, const void *const *src, const uin
     if (ctx->trace) CK(ctx, cudaEventRecord(s.ev_h0, ctx->st_h2d));
     for (uint32_t i = 0; i < n; i++)
         if (src_len[i]) CK(ctx, cudaMemcpyAsync(s.d_in + in_off[i], src[i], src_len[i], cudaMemcpyHostToDevice, ctx->st_h2d));
-
-    // No MD5 pacing on the host path: paced LZ4 warps keep every CTA resident for the whole MD5 chain (tens of
-    // ms), which would serialise the kernels of different slots; unpaced, a batch's LZ4 CTAs retire in a few ms
-    // and the next slot's kernel overlaps this one's MD5 tail.
     if (e2ee) {
         memcpy(s.h_nonce, nonces, 24ull * n);
         CK(ctx, cudaMemcpyAsync(s.d_nonce, s.h_nonce, 24ull * n, cudaMemcpyHostToDevice, ctx->st_h2d));
     }
     s.flags = flags;
-    int rc = launch_batch(ctx, s, s.stream, ctx->st_h2d, n, s.d_in, in_off.data(), src_len, s.d_out, out_off.data(), flags | SKY_F_NO_PACING);
+    int rc = launch_batch(ctx, s, s.stream, ctx->st_h2d, n, s.d_in, in_off.data(), src_len, s.d_out, out_off.data(), flags);
     if (rc != SKY_OK) return rc;
     s.busy = true;
     s.d2h_issued = false;
@@ -1287,11 +1228,7 @@ static int launch_decode(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, con
     CK(ctx, cudaMemsetAsync(s.d_freed, 0, n * sizeof(uint32_t), st));
     CK(ctx, cudaMemsetAsync(s.d_dstatus, 0, n * sizeof(int32_t), st));
     CK(ctx, cudaMemsetAsync(s.d_blkdone, 0, (nblk_total + 1) * sizeof(uint32_t), st));
-    // MD5 lane assignment: longest chunks first (same rule as the sender side)
-    const uint32_t ng = (n + 31) / 32;
-    std::iota(s.h_order, s.h_order + n, 0u);
-    std::stable_sort(s.h_order, s.h_order + n, [&](uint32_t a, uint32_t b) { return raw_len[a] > raw_len[b]; });
-    for (uint32_t i = n; i < ng * 32; i++) s.h_order[i] = 0xffffffffu;
+    const uint32_t ng = fill_md5_order(s.h_order, n, raw_len);
     CK(ctx, cudaMemcpyAsync(s.d_order, s.h_order, ng * 32 * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     memset(s.h_md5, 0, (size_t)n * 16);
     DecParams p;
@@ -1341,12 +1278,7 @@ int sky_decode_device(sky_ctx *ctx, uint32_t n, const void *d_frames, const uint
 }
 
 int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64_t *frame_len, void *const *dst,
-               const uint64_t *raw_len, int32_t *status, uint8_t *md5, float *kernel_ms) {
-    return sky_decode_flags(ctx, n, frames, frame_len, dst, raw_len, 0, status, md5, kernel_ms);
-}
-
-int sky_decode_flags(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64_t *frame_len, void *const *dst,
-                     const uint64_t *raw_len, uint32_t flags, int32_t *status, uint8_t *md5, float *kernel_ms) {
+               const uint64_t *raw_len, uint32_t flags, int32_t *status, uint8_t *md5, float *kernel_ms) {
     if (!ctx || n == 0 || !frames || !frame_len || !dst || !raw_len) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
     Slot &s = ctx->slots[0];

@@ -14,7 +14,7 @@ LIB_PATH = _PKG / "libskychunk.so"
 
 SKY_OK = 0
 SKY_E_INVALID, SKY_E_NOGPU, SKY_E_CUDA, SKY_E_CAPACITY, SKY_E_BUSY, SKY_E_TICKET, SKY_E_NOMEM, SKY_E_NOKEY = -1, -2, -3, -4, -5, -6, -7, -8
-F_LZ4, F_MD5, F_MD5_EXCLUSIVE, F_NO_PACING, F_E2EE = 1, 2, 4, 8, 16
+F_LZ4, F_MD5, F_E2EE = 1, 2, 16
 BOX_OVERHEAD = 40
 # sky_decode status codes
 D_OK, D_BAD_HEADER, D_CORRUPT, D_SIZE, D_UNSUPPORTED, D_LAYOUT, D_TRUNCATED, D_AUTH = 0, -1, -2, -3, -4, -5, -6, -7
@@ -25,8 +25,7 @@ D_NAMES = {0: "ok", -1: "bad frame header", -2: "corrupt block", -3: "size misma
 ABI_SYMBOLS = (
     "sky_strerror", "sky_last_error", "sky_abi_version", "sky_device_count", "sky_device_pci_bus_id", "sky_kernel_config", "sky_frame_bound",
     "sky_ctx_create", "sky_ctx_destroy", "sky_pinned_alloc", "sky_pinned_free",
-    "sky_submit", "sky_wait", "sky_submit_flags", "sky_set_e2ee_key", "sky_box_bound", "sky_process_device", "sky_decode_device", "sky_decode",
-    "sky_decode_flags",
+    "sky_submit", "sky_wait", "sky_set_e2ee_key", "sky_box_bound", "sky_process_device", "sky_decode_device", "sky_decode",
     "sky_device_alloc", "sky_device_free", "sky_memcpy_h2d", "sky_memcpy_d2h", "sky_launch_count",
 )
 
@@ -90,10 +89,8 @@ def lib() -> ctypes.CDLL:
     L.sky_pinned_alloc.restype = vp
     L.sky_pinned_free.argtypes = [vp]
     L.sky_pinned_free.restype = i32
-    L.sky_submit.argtypes = [vp, u32, ctypes.POINTER(vp), p_u64, ctypes.POINTER(vp), p_u64, p_u64]
+    L.sky_submit.argtypes = [vp, u32, ctypes.POINTER(vp), p_u64, ctypes.POINTER(vp), p_u64, u32, ctypes.c_char_p, p_u64]
     L.sky_submit.restype = i32
-    L.sky_submit_flags.argtypes = [vp, u32, ctypes.POINTER(vp), p_u64, ctypes.POINTER(vp), p_u64, u32, ctypes.c_char_p, p_u64]
-    L.sky_submit_flags.restype = i32
     L.sky_set_e2ee_key.argtypes = [vp, ctypes.c_char_p]
     L.sky_set_e2ee_key.restype = i32
     L.sky_box_bound.argtypes = [u64]
@@ -105,10 +102,8 @@ def lib() -> ctypes.CDLL:
     p_i32 = ctypes.POINTER(ctypes.c_int32)
     L.sky_decode_device.argtypes = [vp, u32, vp, p_u64, p_u64, vp, p_u64, p_u64, vp, p_i32, vp, ctypes.POINTER(ctypes.c_float)]
     L.sky_decode_device.restype = i32
-    L.sky_decode.argtypes = [vp, u32, ctypes.POINTER(vp), p_u64, ctypes.POINTER(vp), p_u64, p_i32, vp, ctypes.POINTER(ctypes.c_float)]
+    L.sky_decode.argtypes = [vp, u32, ctypes.POINTER(vp), p_u64, ctypes.POINTER(vp), p_u64, u32, p_i32, vp, ctypes.POINTER(ctypes.c_float)]
     L.sky_decode.restype = i32
-    L.sky_decode_flags.argtypes = [vp, u32, ctypes.POINTER(vp), p_u64, ctypes.POINTER(vp), p_u64, u32, p_i32, vp, ctypes.POINTER(ctypes.c_float)]
-    L.sky_decode_flags.restype = i32
     L.sky_device_alloc.argtypes = [vp, u64, ctypes.POINTER(vp)]
     L.sky_device_alloc.restype = i32
     L.sky_device_free.argtypes = [vp, vp]
@@ -238,7 +233,7 @@ class Context:
         if nonces is not None and len(nonces) != 24 * n:
             raise ValueError("need 24 nonce bytes per chunk")
         t = ctypes.c_uint64(0)
-        self._check(lib().sky_submit_flags(self._h, n, args[0], args[1], args[2], args[3], flags, nonces, ctypes.byref(t)))
+        self._check(lib().sky_submit(self._h, n, args[0], args[1], args[2], args[3], flags, nonces, ctypes.byref(t)))
         self._inflight[t.value] = (n, args)  # keep the pointer arrays alive until wait()
         return t.value
 
@@ -290,7 +285,7 @@ class Context:
         st = (ctypes.c_int32 * n)()
         md5 = (ctypes.c_ubyte * (16 * n))()
         ms = ctypes.c_float(0)
-        self._check(lib().sky_decode_flags(self._h, n, A(*frame_addrs), U(*frame_lens), A(*dst_addrs), U(*raw_lens), flags, st, md5, ctypes.byref(ms)))
+        self._check(lib().sky_decode(self._h, n, A(*frame_addrs), U(*frame_lens), A(*dst_addrs), U(*raw_lens), flags, st, md5, ctypes.byref(ms)))
         raw = bytes(md5)
         return list(st), [raw[16 * i : 16 * i + 16] for i in range(n)], ms.value
 

@@ -225,19 +225,15 @@ def test_run_to_run_determinism(ctx):
     assert a == b
 
 
-def test_stage_flags(ctx):
+def test_stage_flags_lz4_md5_both(ctx):
     datas = [synth.silesia_like_chunk(2, 1 << 20), b"abc"]
     frames, digests, lens, _ = run_device(ctx, datas, flags=native.F_LZ4)
     for d, f in zip(datas, frames):
         check_frame(f, d)
     assert all(dg == bytes(16) for dg in digests)  # MD5 stage not run
-    _, digests, lens, _ = run_device(ctx, datas, flags=native.F_MD5 | native.F_MD5_EXCLUSIVE)
+    _, digests, lens, _ = run_device(ctx, datas, flags=native.F_MD5)
     assert [dg for dg in digests] == [hashlib.md5(d).digest() for d in datas] and all(l == 0 for l in lens)
-    frames, digests, _, _ = run_device(ctx, datas, flags=native.F_LZ4 | native.F_MD5 | native.F_NO_PACING)
-    for d, f, dg in zip(datas, frames, digests):
-        check_frame(f, d)
-        assert dg == hashlib.md5(d).digest()
-    frames, digests, _, _ = run_device(ctx, datas, flags=native.F_LZ4 | native.F_MD5 | native.F_MD5_EXCLUSIVE)
+    frames, digests, _, _ = run_device(ctx, datas, flags=native.F_LZ4 | native.F_MD5)
     for d, f, dg in zip(datas, frames, digests):
         check_frame(f, d)
         assert dg == hashlib.md5(d).digest()

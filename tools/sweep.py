@@ -41,13 +41,12 @@ def main():
     ap.add_argument("--total-mib", type=int, default=2048)
     ap.add_argument("--sizes-mib", default="8")
     ap.add_argument("--workloads", default="random,silesia")
-    ap.add_argument("--flags", default="lz4,md5,both,both_excl")
+    ap.add_argument("--flags", default="lz4,md5,both")
     ap.add_argument("--iters", type=int, default=3)
     ap.add_argument("--decode", action="store_true", help="also time the receiver-side decode + MD5 of the frames")
     a = ap.parse_args()
     dev = torch.device("cuda", 0)
-    FL = {"lz4": native.F_LZ4, "md5": native.F_MD5, "both": 0, "both_excl": native.F_MD5_EXCLUSIVE, "md5_excl": native.F_MD5 | native.F_MD5_EXCLUSIVE,
-          "both_nopace": native.F_NO_PACING}
+    FL = {"lz4": native.F_LZ4, "md5": native.F_MD5, "both": 0}
     for wl in a.workloads.split(","):
         for sz in a.sizes_mib.split(","):
             chunk_bytes = int(float(sz) * (1 << 20))
