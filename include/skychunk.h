@@ -42,7 +42,7 @@ extern "C" {
 #define SKY_E_INVALID (-1)   /* bad argument (null pointer, misaligned device pointer, n == 0 ...) */
 #define SKY_E_NOGPU (-2)     /* no CUDA device / driver: there is NO CPU fallback */
 #define SKY_E_CUDA (-3)      /* a CUDA call failed; see sky_last_error() */
-#define SKY_E_CAPACITY (-4)  /* batch exceeds what the ctx was created for, or dst_cap < sky_frame_bound() */
+#define SKY_E_CAPACITY (-4)  /* batch exceeds what the ctx was created for, dst_cap < sky_frame_bound(), or a chunk > 128 GiB */
 #define SKY_E_BUSY (-5)      /* all slots hold un-waited tickets */
 #define SKY_E_TICKET (-6)    /* unknown / already consumed ticket */
 #define SKY_E_NOMEM (-7)

@@ -11,6 +11,7 @@
 #include <stdint.h>
 
 #include <type_traits>
+#include <utility>
 
 #ifndef SKY_MD5_SLOTS
 #define SKY_MD5_SLOTS 4
@@ -46,89 +47,125 @@ __device__ __forceinline__ uint32_t md5_mk(uint32_t m, uint32_t k) {
 #define SKY_H(b, c, d) ((b) ^ (c) ^ (d))
 #define SKY_I(b, c, d) ((c) ^ ((b) | ~(d)))
 
-// One 64-byte block.  w[16] = little-endian message words.
+// Round R (16 steps) of one 64-byte block on the working state; w[16] = little-endian message words.  md5_warp
+// interleaves its staging between the rounds, so they are separate functions.
+template <int R>
+__device__ __forceinline__ void md5_round(uint32_t &a, uint32_t &b, uint32_t &c, uint32_t &d, const uint32_t (&w)[16]) {
+    if constexpr (R == 0) {
+        SKY_MD5_STEP(SKY_F, a, b, c, d, w[0], 0xd76aa478, 7)
+        SKY_MD5_STEP(SKY_F, d, a, b, c, w[1], 0xe8c7b756, 12)
+        SKY_MD5_STEP(SKY_F, c, d, a, b, w[2], 0x242070db, 17)
+        SKY_MD5_STEP(SKY_F, b, c, d, a, w[3], 0xc1bdceee, 22)
+        SKY_MD5_STEP(SKY_F, a, b, c, d, w[4], 0xf57c0faf, 7)
+        SKY_MD5_STEP(SKY_F, d, a, b, c, w[5], 0x4787c62a, 12)
+        SKY_MD5_STEP(SKY_F, c, d, a, b, w[6], 0xa8304613, 17)
+        SKY_MD5_STEP(SKY_F, b, c, d, a, w[7], 0xfd469501, 22)
+        SKY_MD5_STEP(SKY_F, a, b, c, d, w[8], 0x698098d8, 7)
+        SKY_MD5_STEP(SKY_F, d, a, b, c, w[9], 0x8b44f7af, 12)
+        SKY_MD5_STEP(SKY_F, c, d, a, b, w[10], 0xffff5bb1, 17)
+        SKY_MD5_STEP(SKY_F, b, c, d, a, w[11], 0x895cd7be, 22)
+        SKY_MD5_STEP(SKY_F, a, b, c, d, w[12], 0x6b901122, 7)
+        SKY_MD5_STEP(SKY_F, d, a, b, c, w[13], 0xfd987193, 12)
+        SKY_MD5_STEP(SKY_F, c, d, a, b, w[14], 0xa679438e, 17)
+        SKY_MD5_STEP(SKY_F, b, c, d, a, w[15], 0x49b40821, 22)
+    } else if constexpr (R == 1) {
+        SKY_MD5_STEP(SKY_G, a, b, c, d, w[1], 0xf61e2562, 5)
+        SKY_MD5_STEP(SKY_G, d, a, b, c, w[6], 0xc040b340, 9)
+        SKY_MD5_STEP(SKY_G, c, d, a, b, w[11], 0x265e5a51, 14)
+        SKY_MD5_STEP(SKY_G, b, c, d, a, w[0], 0xe9b6c7aa, 20)
+        SKY_MD5_STEP(SKY_G, a, b, c, d, w[5], 0xd62f105d, 5)
+        SKY_MD5_STEP(SKY_G, d, a, b, c, w[10], 0x02441453, 9)
+        SKY_MD5_STEP(SKY_G, c, d, a, b, w[15], 0xd8a1e681, 14)
+        SKY_MD5_STEP(SKY_G, b, c, d, a, w[4], 0xe7d3fbc8, 20)
+        SKY_MD5_STEP(SKY_G, a, b, c, d, w[9], 0x21e1cde6, 5)
+        SKY_MD5_STEP(SKY_G, d, a, b, c, w[14], 0xc33707d6, 9)
+        SKY_MD5_STEP(SKY_G, c, d, a, b, w[3], 0xf4d50d87, 14)
+        SKY_MD5_STEP(SKY_G, b, c, d, a, w[8], 0x455a14ed, 20)
+        SKY_MD5_STEP(SKY_G, a, b, c, d, w[13], 0xa9e3e905, 5)
+        SKY_MD5_STEP(SKY_G, d, a, b, c, w[2], 0xfcefa3f8, 9)
+        SKY_MD5_STEP(SKY_G, c, d, a, b, w[7], 0x676f02d9, 14)
+        SKY_MD5_STEP(SKY_G, b, c, d, a, w[12], 0x8d2a4c8a, 20)
+    } else if constexpr (R == 2) {
+        SKY_MD5_STEP(SKY_H, a, b, c, d, w[5], 0xfffa3942, 4)
+        SKY_MD5_STEP(SKY_H, d, a, b, c, w[8], 0x8771f681, 11)
+        SKY_MD5_STEP(SKY_H, c, d, a, b, w[11], 0x6d9d6122, 16)
+        SKY_MD5_STEP(SKY_H, b, c, d, a, w[14], 0xfde5380c, 23)
+        SKY_MD5_STEP(SKY_H, a, b, c, d, w[1], 0xa4beea44, 4)
+        SKY_MD5_STEP(SKY_H, d, a, b, c, w[4], 0x4bdecfa9, 11)
+        SKY_MD5_STEP(SKY_H, c, d, a, b, w[7], 0xf6bb4b60, 16)
+        SKY_MD5_STEP(SKY_H, b, c, d, a, w[10], 0xbebfbc70, 23)
+        SKY_MD5_STEP(SKY_H, a, b, c, d, w[13], 0x289b7ec6, 4)
+        SKY_MD5_STEP(SKY_H, d, a, b, c, w[0], 0xeaa127fa, 11)
+        SKY_MD5_STEP(SKY_H, c, d, a, b, w[3], 0xd4ef3085, 16)
+        SKY_MD5_STEP(SKY_H, b, c, d, a, w[6], 0x04881d05, 23)
+        SKY_MD5_STEP(SKY_H, a, b, c, d, w[9], 0xd9d4d039, 4)
+        SKY_MD5_STEP(SKY_H, d, a, b, c, w[12], 0xe6db99e5, 11)
+        SKY_MD5_STEP(SKY_H, c, d, a, b, w[15], 0x1fa27cf8, 16)
+        SKY_MD5_STEP(SKY_H, b, c, d, a, w[2], 0xc4ac5665, 23)
+    } else {
+        SKY_MD5_STEP(SKY_I, a, b, c, d, w[0], 0xf4292244, 6)
+        SKY_MD5_STEP(SKY_I, d, a, b, c, w[7], 0x432aff97, 10)
+        SKY_MD5_STEP(SKY_I, c, d, a, b, w[14], 0xab9423a7, 15)
+        SKY_MD5_STEP(SKY_I, b, c, d, a, w[5], 0xfc93a039, 21)
+        SKY_MD5_STEP(SKY_I, a, b, c, d, w[12], 0x655b59c3, 6)
+        SKY_MD5_STEP(SKY_I, d, a, b, c, w[3], 0x8f0ccc92, 10)
+        SKY_MD5_STEP(SKY_I, c, d, a, b, w[10], 0xffeff47d, 15)
+        SKY_MD5_STEP(SKY_I, b, c, d, a, w[1], 0x85845dd1, 21)
+        SKY_MD5_STEP(SKY_I, a, b, c, d, w[8], 0x6fa87e4f, 6)
+        SKY_MD5_STEP(SKY_I, d, a, b, c, w[15], 0xfe2ce6e0, 10)
+        SKY_MD5_STEP(SKY_I, c, d, a, b, w[6], 0xa3014314, 15)
+        SKY_MD5_STEP(SKY_I, b, c, d, a, w[13], 0x4e0811a1, 21)
+        SKY_MD5_STEP(SKY_I, a, b, c, d, w[4], 0xf7537e82, 6)
+        SKY_MD5_STEP(SKY_I, d, a, b, c, w[11], 0xbd3af235, 10)
+        SKY_MD5_STEP(SKY_I, c, d, a, b, w[2], 0x2ad7d2bb, 15)
+        SKY_MD5_STEP(SKY_I, b, c, d, a, w[9], 0xeb86d391, 21)
+    }
+}
+
+// One 64-byte block.
 __device__ __forceinline__ void md5_block(Md5State &st, const uint32_t (&w)[16]) {
     uint32_t a = st.a, b = st.b, c = st.c, d = st.d;
-    SKY_MD5_STEP(SKY_F, a, b, c, d, w[0], 0xd76aa478, 7)
-    SKY_MD5_STEP(SKY_F, d, a, b, c, w[1], 0xe8c7b756, 12)
-    SKY_MD5_STEP(SKY_F, c, d, a, b, w[2], 0x242070db, 17)
-    SKY_MD5_STEP(SKY_F, b, c, d, a, w[3], 0xc1bdceee, 22)
-    SKY_MD5_STEP(SKY_F, a, b, c, d, w[4], 0xf57c0faf, 7)
-    SKY_MD5_STEP(SKY_F, d, a, b, c, w[5], 0x4787c62a, 12)
-    SKY_MD5_STEP(SKY_F, c, d, a, b, w[6], 0xa8304613, 17)
-    SKY_MD5_STEP(SKY_F, b, c, d, a, w[7], 0xfd469501, 22)
-    SKY_MD5_STEP(SKY_F, a, b, c, d, w[8], 0x698098d8, 7)
-    SKY_MD5_STEP(SKY_F, d, a, b, c, w[9], 0x8b44f7af, 12)
-    SKY_MD5_STEP(SKY_F, c, d, a, b, w[10], 0xffff5bb1, 17)
-    SKY_MD5_STEP(SKY_F, b, c, d, a, w[11], 0x895cd7be, 22)
-    SKY_MD5_STEP(SKY_F, a, b, c, d, w[12], 0x6b901122, 7)
-    SKY_MD5_STEP(SKY_F, d, a, b, c, w[13], 0xfd987193, 12)
-    SKY_MD5_STEP(SKY_F, c, d, a, b, w[14], 0xa679438e, 17)
-    SKY_MD5_STEP(SKY_F, b, c, d, a, w[15], 0x49b40821, 22)
-
-    SKY_MD5_STEP(SKY_G, a, b, c, d, w[1], 0xf61e2562, 5)
-    SKY_MD5_STEP(SKY_G, d, a, b, c, w[6], 0xc040b340, 9)
-    SKY_MD5_STEP(SKY_G, c, d, a, b, w[11], 0x265e5a51, 14)
-    SKY_MD5_STEP(SKY_G, b, c, d, a, w[0], 0xe9b6c7aa, 20)
-    SKY_MD5_STEP(SKY_G, a, b, c, d, w[5], 0xd62f105d, 5)
-    SKY_MD5_STEP(SKY_G, d, a, b, c, w[10], 0x02441453, 9)
-    SKY_MD5_STEP(SKY_G, c, d, a, b, w[15], 0xd8a1e681, 14)
-    SKY_MD5_STEP(SKY_G, b, c, d, a, w[4], 0xe7d3fbc8, 20)
-    SKY_MD5_STEP(SKY_G, a, b, c, d, w[9], 0x21e1cde6, 5)
-    SKY_MD5_STEP(SKY_G, d, a, b, c, w[14], 0xc33707d6, 9)
-    SKY_MD5_STEP(SKY_G, c, d, a, b, w[3], 0xf4d50d87, 14)
-    SKY_MD5_STEP(SKY_G, b, c, d, a, w[8], 0x455a14ed, 20)
-    SKY_MD5_STEP(SKY_G, a, b, c, d, w[13], 0xa9e3e905, 5)
-    SKY_MD5_STEP(SKY_G, d, a, b, c, w[2], 0xfcefa3f8, 9)
-    SKY_MD5_STEP(SKY_G, c, d, a, b, w[7], 0x676f02d9, 14)
-    SKY_MD5_STEP(SKY_G, b, c, d, a, w[12], 0x8d2a4c8a, 20)
-
-    SKY_MD5_STEP(SKY_H, a, b, c, d, w[5], 0xfffa3942, 4)
-    SKY_MD5_STEP(SKY_H, d, a, b, c, w[8], 0x8771f681, 11)
-    SKY_MD5_STEP(SKY_H, c, d, a, b, w[11], 0x6d9d6122, 16)
-    SKY_MD5_STEP(SKY_H, b, c, d, a, w[14], 0xfde5380c, 23)
-    SKY_MD5_STEP(SKY_H, a, b, c, d, w[1], 0xa4beea44, 4)
-    SKY_MD5_STEP(SKY_H, d, a, b, c, w[4], 0x4bdecfa9, 11)
-    SKY_MD5_STEP(SKY_H, c, d, a, b, w[7], 0xf6bb4b60, 16)
-    SKY_MD5_STEP(SKY_H, b, c, d, a, w[10], 0xbebfbc70, 23)
-    SKY_MD5_STEP(SKY_H, a, b, c, d, w[13], 0x289b7ec6, 4)
-    SKY_MD5_STEP(SKY_H, d, a, b, c, w[0], 0xeaa127fa, 11)
-    SKY_MD5_STEP(SKY_H, c, d, a, b, w[3], 0xd4ef3085, 16)
-    SKY_MD5_STEP(SKY_H, b, c, d, a, w[6], 0x04881d05, 23)
-    SKY_MD5_STEP(SKY_H, a, b, c, d, w[9], 0xd9d4d039, 4)
-    SKY_MD5_STEP(SKY_H, d, a, b, c, w[12], 0xe6db99e5, 11)
-    SKY_MD5_STEP(SKY_H, c, d, a, b, w[15], 0x1fa27cf8, 16)
-    SKY_MD5_STEP(SKY_H, b, c, d, a, w[2], 0xc4ac5665, 23)
-
-    SKY_MD5_STEP(SKY_I, a, b, c, d, w[0], 0xf4292244, 6)
-    SKY_MD5_STEP(SKY_I, d, a, b, c, w[7], 0x432aff97, 10)
-    SKY_MD5_STEP(SKY_I, c, d, a, b, w[14], 0xab9423a7, 15)
-    SKY_MD5_STEP(SKY_I, b, c, d, a, w[5], 0xfc93a039, 21)
-    SKY_MD5_STEP(SKY_I, a, b, c, d, w[12], 0x655b59c3, 6)
-    SKY_MD5_STEP(SKY_I, d, a, b, c, w[3], 0x8f0ccc92, 10)
-    SKY_MD5_STEP(SKY_I, c, d, a, b, w[10], 0xffeff47d, 15)
-    SKY_MD5_STEP(SKY_I, b, c, d, a, w[1], 0x85845dd1, 21)
-    SKY_MD5_STEP(SKY_I, a, b, c, d, w[8], 0x6fa87e4f, 6)
-    SKY_MD5_STEP(SKY_I, d, a, b, c, w[15], 0xfe2ce6e0, 10)
-    SKY_MD5_STEP(SKY_I, c, d, a, b, w[6], 0xa3014314, 15)
-    SKY_MD5_STEP(SKY_I, b, c, d, a, w[13], 0x4e0811a1, 21)
-    SKY_MD5_STEP(SKY_I, a, b, c, d, w[4], 0xf7537e82, 6)
-    SKY_MD5_STEP(SKY_I, d, a, b, c, w[11], 0xbd3af235, 10)
-    SKY_MD5_STEP(SKY_I, c, d, a, b, w[2], 0x2ad7d2bb, 15)
-    SKY_MD5_STEP(SKY_I, b, c, d, a, w[9], 0xeb86d391, 21)
+    md5_round<0>(a, b, c, d, w);
+    md5_round<1>(a, b, c, d, w);
+    md5_round<2>(a, b, c, d, w);
+    md5_round<3>(a, b, c, d, w);
     st.a += a;
     st.b += b;
     st.c += c;
     st.d += d;
 }
 
-__device__ __forceinline__ void cp_async16(uint32_t smem_addr, const void *gptr) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(smem_addr), "l"(gptr) : "memory");
+// Stages one 64-byte block from `gptr` into ring slot `kSlot` of this lane (`lane_ring` = shared address of the lane's
+// piece 0 of slot 0; pieces are 512 B apart, slots 2 KiB), if `pred`.  The predicate is applied inside the asm, so no
+// branch goes around the copies, and the slot offsets are immediates.
+template <int kSlot>
+__device__ __forceinline__ void cp_async_block(bool pred, uint32_t lane_ring, const uint8_t *gptr) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %2, 0;\n\t"
+        "@p cp.async.cg.shared.global [%0+%3], [%1], 16;\n\t"
+        "@p cp.async.cg.shared.global [%0+%4], [%1+16], 16;\n\t"
+        "@p cp.async.cg.shared.global [%0+%5], [%1+32], 16;\n\t"
+        "@p cp.async.cg.shared.global [%0+%6], [%1+48], 16;\n\t}" ::"r"(lane_ring),
+        "l"(gptr), "r"((uint32_t)pred), "n"(kSlot * 2048), "n"(kSlot * 2048 + 512), "n"(kSlot * 2048 + 1024),
+        "n"(kSlot * 2048 + 1536)
+        : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory");
+}
+
+// f(std::integral_constant<int, 0>()), ..., f(std::integral_constant<int, N - 1>()): an unrolled loop whose index is a
+// constant expression (ring slots are template arguments of cp_async_block).
+template <class F, int... I>
+__device__ __forceinline__ void md5_unroll_(F &&f, std::integer_sequence<int, I...>) {
+    (f(std::integral_constant<int, I>()), ...);
+}
+template <int N, class F>
+__device__ __forceinline__ void md5_unroll(F &&f) {
+    md5_unroll_(f, std::make_integer_sequence<int, N>());
 }
 
 // Digest of one chunk per lane.  `ring` = this warp's 8 KiB shared-memory area (2048 x uint32),
@@ -144,77 +181,86 @@ template <class Gate = Md5NoGate>
 __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uint64_t len, bool active, uint8_t *out,
                                          unsigned lane, Gate gate = Gate()) {
     constexpr int kSlots = SKY_MD5_SLOTS;  // ring depth (blocks, power of two); prefetch distance = kSlots - 1
+    static_assert(kSlots >= 2 && (kSlots & (kSlots - 1)) == 0 && 1024 % kSlots == 0, "SKY_MD5_SLOTS: a power of two, 2..1024");
     constexpr bool kGated = !std::is_same<Gate, Md5NoGate>::value;
-    const uint64_t nfull = active ? (len >> 6) : 0;
-    uint64_t wmax = nfull;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        uint64_t other = __shfl_xor_sync(0xffffffffu, wmax, o);
-        wmax = other > wmax ? other : wmax;
-    }
-    Md5State st;
+    // Block counts are 32-bit: the host rejects chunks over 128 GiB (kMaxChunkBlocks in skychunk.cu), so nfull <= 2^31
+    // and the trip count rounded up to kSlots cannot wrap.
+    const uint32_t nfull = active ? (uint32_t)(len >> 6) : 0;
+    const uint32_t wmax = __reduce_max_sync(0xffffffffu, nfull);
+    const uint32_t trips = (wmax + (kSlots - 1)) & ~(uint32_t)(kSlots - 1);
+    Md5State st;  // runs on through the blocks past this lane's end (the loop has no branch per lane) ...
     md5_init(st);
-    const uint32_t ring_base = (uint32_t)__cvta_generic_to_shared(ring);
-    // slot s, piece q of this lane lives at ring[((s*4 + q)*32 + lane) * 4 words]
-    auto slot_addr = [&](int s, int q) { return ring_base + (uint32_t)(((s * 4 + q) * 32 + lane) * 16); };
+    Md5State fin = st;  // ... so the state after the lane's last full block is kept here, off the chain
+    // slot s, piece q of this lane lives at ring[((s*4 + q)*32 + lane) * 4 words]: a per-lane base plus an immediate
+    const uint32_t *lring = ring + lane * 4;
+    const uint32_t lring_s = (uint32_t)__cvta_generic_to_shared(lring);
 
     gate(0, active && len > 0);
-#pragma unroll
-    for (int s = 0; s < kSlots - 1; s++) {
-        if ((uint64_t)s < nfull) {
-#pragma unroll
-            for (int q = 0; q < 4; q++) cp_async16(slot_addr(s, q), src + (uint64_t)s * 64 + q * 16);
-        }
+    md5_unroll<kSlots - 1>([&](auto sc) {
+        constexpr int s = decltype(sc)::value;
+        cp_async_block<s>((uint32_t)s < nfull, lring_s, src + s * 64);
         cp_async_commit();
-    }
+    });
     auto load_words = [&](uint32_t (&w)[16], int cs) {
 #pragma unroll
         for (int q = 0; q < 4; q++) {
-            const uint4 v = *reinterpret_cast<const uint4 *>(ring + ((cs * 4 + q) * 32 + lane) * 4);
+            const uint4 v = *reinterpret_cast<const uint4 *>(lring + (cs * 4 + q) * 128);
             w[4 * q + 0] = v.x;
             w[4 * q + 1] = v.y;
             w[4 * q + 2] = v.z;
             w[4 * q + 3] = v.w;
         }
     };
-    // software pipeline: the words of block i+1 are pulled from the ring (LDS) while block i's chain runs
-    uint32_t wn[16];
-#pragma unroll
-    for (int k = 0; k < 16; k++) wn[k] = 0;
+    // Software pipeline over two word buffers: the words of block i+1 are pulled from the ring (LDS) while block i's
+    // chain runs.  Every lane hashes every block up to `trips`; a lane past its end hashes stale ring words and keeps
+    // only `fin`.
+    uint32_t w[2][16];
     cp_async_wait<kSlots - 2>();  // block 0 has landed
-    if (nfull) load_words(wn, 0);
-#define SKY_MD5_LOOP_BODY(i)                                                                              \
-    {                                                                                                     \
-        uint32_t w[16];                                                                                   \
-        _Pragma("unroll") for (int k = 0; k < 16; k++) w[k] = wn[k];                                      \
-        const uint64_t pf = (i) + (kSlots - 1);                                                           \
-        if (pf < nfull) {                                                                                 \
-            const int ps = (int)(pf & (kSlots - 1)); /* == slot of block i-1, last read one iteration ago */ \
-            _Pragma("unroll") for (int q = 0; q < 4; q++) cp_async16(slot_addr(ps, q), src + pf * 64 + q * 16); \
-        }                                                                                                 \
-        cp_async_commit();                                                                                \
-        cp_async_wait<kSlots - 2>(); /* block i+1 has landed */                                           \
-        if ((i) + 1 < nfull) load_words(wn, (int)(((i) + 1) & (kSlots - 1)));                             \
-        if ((i) < nfull) md5_block(st, w);                                                                \
-    }
+    load_words(w[0], 0);
+    const uint8_t *pf_src = src + (kSlots - 1) * 64;  // block i + kSlots - 1, the next one to stage
+    // Blocks i .. i + kSlots - 1 (i a multiple of kSlots) as one branch-free stretch: the staging sits between the
+    // rounds, where ptxas can issue it in the chain's idle cycles.
+    auto blocks = [&](uint32_t i) {
+        md5_unroll<kSlots>([&](auto uc) {
+            constexpr int u = decltype(uc)::value;
+            constexpr int ps = (u + kSlots - 1) & (kSlots - 1);  // slot of block i+u-1, read during block i+u-2
+            constexpr int ns = (u + 1) & (kSlots - 1);
+            uint32_t a = st.a, b = st.b, c = st.c, d = st.d;
+            md5_round<0>(a, b, c, d, w[u & 1]);
+            cp_async_block<ps>(i + u + (kSlots - 1) < nfull, lring_s, pf_src + u * 64);
+            md5_round<1>(a, b, c, d, w[u & 1]);
+            cp_async_commit();
+            cp_async_wait<kSlots - 2>();  // block i+u+1 has landed
+            md5_round<2>(a, b, c, d, w[u & 1]);
+            load_words(w[(u + 1) & 1], ns);
+            md5_round<3>(a, b, c, d, w[u & 1]);
+            st.a += a;
+            st.b += b;
+            st.c += c;
+            st.d += d;
+            if (i + u < nfull) fin = st;
+        });
+        pf_src += kSlots * 64;
+    };
     if constexpr (kGated) {
         // Receiver side: a row-granular outer loop keeps the gate (a spin with a scheduling barrier) out of the
-        // chain-bound inner loop; the prefetch runs kSlots-1 blocks ahead, so a row is gated one row early.
-        for (uint64_t base = 0; base < wmax; base += 1024) {
-            gate((base >> 10) + 1, (base + 1024) * 64 < len);
-            const uint64_t iend = (wmax - base > 1024) ? base + 1024 : wmax;
-            for (uint64_t i = base; i < iend; i++) SKY_MD5_LOOP_BODY(i)
+        // chain-bound inner loop; the prefetch runs kSlots-1 blocks ahead, so a row is gated one row early.  A row
+        // (1024 blocks) is a whole number of kSlots-block stretches.
+        for (uint32_t base = 0; base < trips; base += 1024) {
+            gate((base >> 10) + 1, (uint64_t)(base + 1024) * 64 < len);
+            const uint32_t iend = min(base + 1024, trips);
+            for (uint32_t i = base; i < iend; i += kSlots) blocks(i);
         }
     } else {
         // Sender side: one flat loop (measured 1.027x faster per block than the nested form).
-        for (uint64_t i = 0; i < wmax; i++) SKY_MD5_LOOP_BODY(i)
+        for (uint32_t i = 0; i < trips; i += kSlots) blocks(i);
     }
-#undef SKY_MD5_LOOP_BODY
     cp_async_wait<0>();
+    st = fin;
     if (active) {
         // tail: rem bytes + 0x80 + zeros + u64le bit length -> one or two more blocks (slow path, once per chunk)
         const uint32_t rem = (uint32_t)(len & 63);
-        const uint8_t *tp = src + (nfull << 6);
+        const uint8_t *tp = src + ((uint64_t)nfull << 6);
         uint32_t tw[32];
 #pragma unroll
         for (int k = 0; k < 32; k++) tw[k] = 0;

@@ -57,6 +57,7 @@ constexpr int kMd5WarpsPerCta = 4;        // digest CTAs run 4 MD5 groups (one p
 constexpr uint32_t kRingBytes = SKY_MD5_SLOTS * 2048;  // MD5 staging ring: slots x 64 B x 32 lanes
 constexpr uint32_t kLoadPiece = 8192;     // bytes per bulk copy of the block load
 constexpr int kCtasPerSm = 2;             // fused kernel: 2 x ~110 KiB of shared memory per SM
+constexpr uint64_t kMaxChunkBlocks = 1ull << 21;  // 64 KiB blocks = 128 GiB per chunk: md5_warp counts 64-byte blocks in 32 bits
 constexpr int kOffBits = 40;
 constexpr uint64_t kOffMask = (1ull << kOffBits) - 1;
 
@@ -121,6 +122,11 @@ __device__ __forceinline__ uint64_t ld_acquire(const uint64_t *p) {
 __device__ __forceinline__ uint32_t ld_acquire32(const uint32_t *p) {
     uint32_t v;
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint32_t ld_relaxed32(const uint32_t *p) {
+    uint32_t v;
+    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
 }
 __device__ __forceinline__ void st_release(uint64_t *p, uint64_t v) {
@@ -507,13 +513,16 @@ __global__ void sky_frame_index_kernel(const DecParams p) {
 struct DecRowGate {
     const uint32_t *flags;  // this lane's chunk: one word per block, non-zero = decoded (or failed: hash garbage, status says so)
     __device__ __forceinline__ void operator()(uint64_t row, bool wants) const {
+        // Poll with relaxed loads and acquire once: an acquire load at gpu scope invalidates the SM's L1 (CCTL.IVALL),
+        // and an MD5 lane waiting on the decoder polls thousands of times, under the decode warps of its SM.
         unsigned ns = 128;
         for (;;) {
-            const bool ready = !wants || ld_acquire32(flags + row) != 0;
+            const bool ready = !wants || ld_relaxed32(flags + row) != 0;
             if (__all_sync(kFull, ready)) break;
             __nanosleep(ns);
             if (ns < 4096) ns <<= 1;
         }
+        asm volatile("fence.acq_rel.gpu;" ::: "memory");
     }
 };
 
@@ -977,7 +986,7 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
         d.dst = d_dst + dst_off[i];
         d.len = src_len[i];
         const uint64_t nb = (src_len[i] + kBlock - 1) / kBlock;
-        if (nb >= (1ull << 24)) return SKY_E_CAPACITY;
+        if (nb > kMaxChunkBlocks) return SKY_E_CAPACITY;
         d.nblk = (uint32_t)nb;
         rows = std::max(rows, d.nblk);
         s.h_chain[i] = 15;  // block 0 starts right after the 15-byte frame header
@@ -1204,7 +1213,7 @@ static int launch_decode(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, con
         d.frame_len = frame_len[i];
         d.raw_len = raw_len[i];
         const uint64_t nb = (raw_len[i] + kBlock - 1) / kBlock;
-        if (nb >= (1ull << 24)) return SKY_E_CAPACITY;
+        if (nb > kMaxChunkBlocks) return SKY_E_CAPACITY;
         d.nblk = (uint32_t)nb;
         d.blk_base = nblk_total;
         d.linked = 0;

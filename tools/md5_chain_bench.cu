@@ -4,10 +4,17 @@
 //   V0: plain C (ptxas picks IMAD.IADD for the on-chain add: alu -> fma -> alu)
 //   V1: on-chain add forced onto the ALU pipe by consuming its carry (IADD3 with carry-out)
 //   V2: 3-input on-chain add (a, m+K, f) kept separate via carry trick on the inner add
-// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bin/md5_chain_bench tools/md5_chain_bench.cu
+// and, next to them, the product loop itself ("in-situ"): sky::md5_warp from md5.cuh in the flagship's arrangement --
+// one MD5 warp per CTA, 32 CTAs, each lane streaming its own 8 MiB region of one device buffer through the staging ring
+// in dynamic shared memory -- so the gap between the register-only chain and the real loop is measured, not inferred.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I skyplane_b200/csrc \
+//            -o tools/bin/md5_chain_bench tools/md5_chain_bench.cu
+// (-I another directory holding an md5.cuh measures that version of md5_warp; the first argument labels the lines.)
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
+
+#include "md5.cuh"
 
 #define F_(b, c, d) ((d) ^ ((b) & ((c) ^ (d))))
 #define G_(b, c, d) ((c) ^ ((d) & ((b) ^ (c))))
@@ -105,7 +112,82 @@ void run(const char *name, int warps_per_cta, int ctas) {
     cudaFree(cyc);
 }
 
-int main() {
+// ---- in-situ: the product's md5_warp ------------------------------------------------------------------------
+constexpr int kInsituCtas = 32;                 // 1024 chunks = 32 MD5 groups, one per digest CTA
+constexpr uint64_t kInsituLaneBytes = 8 << 20;  // 8 MiB per lane (chunk)
+constexpr uint32_t kInsituRingBytes = SKY_MD5_SLOTS * 2048;
+
+__global__ void fill(uint64_t *p, uint64_t n, uint64_t seed) {
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        uint64_t z = seed + (i + 1) * 0x9e3779b97f4a7c15ull;  // splitmix64
+        z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+        z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+        p[i] = z ^ (z >> 31);
+    }
+}
+
+// __launch_bounds__ as sky_fused_kernel's, so md5_warp is compiled under the same register budget.
+// Lengths and `active` come from device memory, as the fused kernel reads them from its chunk table: constants here
+// let ptxas compile a different loop (without the per-lane branches the fused kernel's copy has).
+__global__ void __launch_bounds__(448, 2) insitu(const uint8_t *buf, const uint64_t *lens, uint8_t *digests, long long *cycles) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const unsigned lane = threadIdx.x & 31;
+    const uint64_t c = (uint64_t)blockIdx.x * 32 + lane;
+    const uint64_t len = lens[c];
+    __syncwarp();
+    const long long t0 = clock64();
+    sky::md5_warp(reinterpret_cast<uint32_t *>(smem), buf + c * kInsituLaneBytes, len, len != 0, digests + c * 16, lane);
+    __syncwarp();
+    const long long t1 = clock64();
+    if (lane == 0) cycles[blockIdx.x] = t1 - t0;
+}
+
+void run_insitu(const char *label) {
+    const uint64_t bytes = kInsituLaneBytes * 32 * kInsituCtas;
+    uint8_t *buf, *dg;
+    uint64_t *lens;
+    long long *cyc;
+    cudaMalloc(&buf, bytes);
+    cudaMalloc(&lens, sizeof(uint64_t) * 32 * kInsituCtas);
+    uint64_t h_lens[32 * kInsituCtas];
+    for (uint64_t &l : h_lens) l = kInsituLaneBytes;
+    cudaMemcpy(lens, h_lens, sizeof h_lens, cudaMemcpyHostToDevice);
+    cudaMalloc(&dg, 16 * 32 * kInsituCtas);
+    cudaMalloc(&cyc, sizeof(long long) * kInsituCtas);
+    fill<<<1024, 256>>>(reinterpret_cast<uint64_t *>(buf), bytes / 8, 1);
+    cudaEvent_t e0, e1;
+    cudaEventCreate(&e0);
+    cudaEventCreate(&e1);
+    const double nblocks = (double)(kInsituLaneBytes / 64);
+    insitu<<<kInsituCtas, 32, kInsituRingBytes>>>(buf, lens, dg, cyc);  // warm-up
+    for (int rep = 0; rep < 5; rep++) {
+        cudaEventRecord(e0);
+        insitu<<<kInsituCtas, 32, kInsituRingBytes>>>(buf, lens, dg, cyc);
+        cudaEventRecord(e1);
+        cudaError_t err = cudaDeviceSynchronize();
+        if (err != cudaSuccess) {
+            printf("in-situ: %s\n", cudaGetErrorString(err));
+            return;
+        }
+        float ms;
+        cudaEventElapsedTime(&ms, e0, e1);
+        long long c[kInsituCtas];
+        cudaMemcpy(c, cyc, sizeof c, cudaMemcpyDeviceToHost);
+        long long lo = c[0], hi = c[0];
+        for (long long v : c) lo = v < lo ? v : lo, hi = v > hi ? v : hi;
+        printf("in-situ md5_warp [%s] rep %d  ctas=%d lanes=32 MiB/lane=%d  cycles/block=%8.1f (fastest CTA %.1f)  "
+               "cycles/step=%6.2f  per-stream=%.4f GB/s  (%.3f ms)\n",
+               label, rep, kInsituCtas, (int)(kInsituLaneBytes >> 20), hi / nblocks, lo / nblocks, hi / nblocks / 64,
+               kInsituLaneBytes / (ms * 1e-3) / 1e9, ms);
+    }
+    cudaFree(buf);
+    cudaFree(lens);
+    cudaFree(dg);
+    cudaFree(cyc);
+}
+
+int main(int argc, char **argv) {
+    const char *label = argc > 1 ? argv[1] : "md5.cuh";
     int sms = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     printf("SMs=%d\n", sms);
@@ -114,5 +196,6 @@ int main() {
         run<1>("V1 iadd3-carry-on-chain", wpc, sms);
         run<2>("V2 ptxas-free-form", wpc, sms);
     }
+    run_insitu(label);
     return 0;
 }
