@@ -26,6 +26,9 @@ struct BoxChunk {
     uint64_t len;        // message bytes
 };
 
+// XSalsa20 stream blocks (work items of sky_box_xor_kernel) of a `len`-byte message: it starts 32 bytes into block 0.
+__host__ __device__ __forceinline__ uint64_t box_stream_blocks(uint64_t len) { return (len + 32 + 63) / 64; }
+
 __device__ __forceinline__ uint32_t rotl(uint32_t x, int s) { return __funnelshift_l(x, x, s); }
 
 __device__ __forceinline__ void salsa20_rounds(uint32_t (&x)[16]) {
@@ -78,7 +81,7 @@ __global__ void sky_box_keys_kernel(const BoxChunk *chunks, uint32_t n, const ui
 }
 
 // ---- XOR with the XSalsa20 stream.  Work item = (chunk, stream block b): message bytes [64b - 32, 64b + 32).
-// blk_base[c] = first work item of chunk c (prefix sum of ceil((len + 32) / 64)), total items = blk_base[n].
+// blk_base[c] = first work item of chunk c (prefix sum of box_stream_blocks(len)), total items = blk_base[n].
 // seal: src = plaintext msg, dst = box + 40.   open: src = box + 40, dst = msg.
 __global__ void sky_box_xor_kernel(const BoxChunk *chunks, const uint64_t *blk_base, uint32_t n, const uint32_t *sub, int open) {
     const uint64_t total = blk_base[n];

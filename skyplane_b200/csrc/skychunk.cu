@@ -18,20 +18,22 @@
 //
 // The two roles never wait on each other: digest lanes and compressors each read their own input from HBM.
 //
-// Host side: sky_ctx owns a stream, pinned + device metadata arrays, and (optionally) per-slot input /
-// output slabs for the host-buffer path (H2D -> kernel -> D2H on one stream per slot).
+// Host side: sky_ctx owns every stream, event and buffer through move-only owners that release them in their destructors:
+// per slot a kernel stream, batch metadata, the receiver's and the E2EE arrays and (optionally) input / output slabs for
+// the host-buffer path (H2D and D2H on two streams shared by the slots, the kernels on the slot's stream).
 // There is NO CPU fallback anywhere in this file: without a CUDA device every entry point fails.
 
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 #include <new>
 #include <numeric>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/skychunk.h"
@@ -489,7 +491,7 @@ struct DecParams {
     DecChunk *chunks;
     DecBlock *blocks;
     int32_t *status;     // per chunk, 0 = ok (mapped host memory)
-    uint32_t *done;      // per chunk: leading blocks fully decoded (linked frames wait on it)
+    uint32_t *dec_done;  // per chunk: leading blocks fully decoded (linked frames wait on it)
     uint32_t *counter;   // work counter
     uint32_t *blk_done;  // per block: 1 once decoded (gates the MD5 lanes)
     const uint32_t *md5_order;
@@ -564,7 +566,7 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
         if (cd.linked) {  // matches may reach into earlier blocks: decode in order within the chunk
             if (lane == 0) {
                 unsigned ns = 64;
-                while (ld_acquire32(p.done + c) < j) {
+                while (ld_acquire32(p.dec_done + c) < j) {
                     __nanosleep(ns);
                     if (ns < 2048) ns <<= 1;
                 }
@@ -586,13 +588,14 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
         __syncwarp();
         if (lane == 0) {
             __threadfence();
-            if (cd.linked) st_release32(p.done + c, j + 1);
+            if (cd.linked) st_release32(p.dec_done + c, j + 1);
             st_release32(p.blk_done + cd.blk_base + j, 1u);  // lets the MD5 lane of this chunk enter the row
         }
     }
 }
 
-// ---- E2EE glue: describe one box per chunk once the frame lengths exist (they are only known on the device).
+// ---- E2EE glue: describe one box per chunk once the frame lengths exist (they are only known on the device; the open
+// side knows every length before it starts, so its descriptors are built on the host, see launch_open).
 // seal: msg = the chunk's frame (or, without LZ4, its raw bytes), box = box_base + (frame offset in the frame slab) + 64*i + 8,
 // so that box + 40 is 16-byte aligned; the nonce is copied in, out_len becomes the box length.
 __global__ void sky_box_setup_kernel(BoxChunk *bc, uint64_t *blk_base, const ChunkDesc *desc, uint32_t n, uint64_t *out_len,
@@ -612,27 +615,7 @@ __global__ void sky_box_setup_kernel(BoxChunk *bc, uint64_t *blk_base, const Chu
         uint64_t acc = 0;
         for (uint32_t i = 0; i < n; i++) {
             blk_base[i] = acc;
-            acc += (bc[i].len + 32 + 63) / 64;
-        }
-        blk_base[n] = acc;
-    }
-}
-// open: the boxes were copied to box_slab (box i at box_off[i] + 8); the plaintext frame goes to frame_slab + frame_off[i].
-__global__ void sky_box_open_setup_kernel(BoxChunk *bc, uint64_t *blk_base, uint32_t n, const uint64_t *box_off, const uint64_t *box_len,
-                                          const uint64_t *frame_off, uint8_t *frame_slab, uint8_t *box_slab) {
-    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
-        BoxChunk b;
-        b.box = box_slab + box_off[i] + 8;
-        b.msg = frame_slab + frame_off[i];
-        b.len = box_len[i] >= (uint64_t)kBoxOverhead ? box_len[i] - kBoxOverhead : 0;
-        bc[i] = b;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint64_t acc = 0;
-        for (uint32_t i = 0; i < n; i++) {
-            blk_base[i] = acc;
-            acc += (bc[i].len + 32 + 63) / 64;
+            acc += box_stream_blocks(bc[i].len);
         }
         blk_base[n] = acc;
     }
@@ -643,64 +626,106 @@ __global__ void sky_box_open_setup_kernel(BoxChunk *bc, uint64_t *blk_base, uint
 // ======================================================================================= host side
 using namespace sky;
 
-struct Slot {
-    cudaStream_t stream = nullptr;
-    uint8_t *d_in = nullptr, *d_out = nullptr;
-    cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr, ev_res = nullptr;  // kernel start / end, results (sizes+digests) on host
-    bool d2h_issued = false;
-    cudaEvent_t ev_h0 = nullptr, ev_d0 = nullptr, ev_d1 = nullptr;  // SKYCHUNK_TRACE only: H2D start, D2H start / end
-    // per-batch metadata (device + pinned host mirrors)
-    ChunkDesc *h_desc = nullptr, *d_desc = nullptr;
-    uint32_t *h_order = nullptr, *d_order = nullptr;
-    uint64_t *h_chain = nullptr, *d_chain = nullptr;
-    uint32_t *d_freed = nullptr;
+// Owner of one CUDA resource (a device or pinned allocation, an event, a stream): move-only, released by its destructor
+// or reset().  put() releases what it holds and hands out the handle a cudaMalloc / cudaEventCreate / ... call fills.
+template <class H, auto Release>
+class Owned {
+    H h_ = nullptr;
+
+  public:
+    Owned() = default;
+    Owned(Owned &&o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+    Owned &operator=(Owned &&o) noexcept { std::swap(h_, o.h_); return *this; }
+    ~Owned() { reset(); }
+    void reset() { if (h_) Release(std::exchange(h_, nullptr)); }
+    H *put() { reset(); return &h_; }
+    operator H() const { return h_; }
+};
+template <class T> using DevMem = Owned<T *, cudaFree>;
+template <class T> using PinnedMem = Owned<T *, cudaFreeHost>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+// Mapped pinned memory: kernels store into it straight over PCIe through `d`, the device view of `h`.
+template <class T>
+struct Mapped {
+    PinnedMem<T> h;
+    T *d = nullptr;
+    cudaError_t alloc(size_t n) {
+        const cudaError_t e = cudaHostAlloc(h.put(), n * sizeof(T), cudaHostAllocMapped | cudaHostAllocPortable);
+        return e == cudaSuccess ? cudaHostGetDevicePointer(&d, h, 0) : e;
+    }
+};
+
+// A slot's memory, one part per role (pinned host mirror h_*, device array d_*).  The batch metadata is built with the
+// slot; the decode and box arrays by the first call that needs them, all of a part or none of it.
+struct BatchMeta {  // one batch's descriptors and results (the receiver uses the MD5 order, digests and counters)
+    PinnedMem<ChunkDesc> h_desc; DevMem<ChunkDesc> d_desc;
+    PinnedMem<uint32_t> h_order; DevMem<uint32_t> d_order;
+    PinnedMem<uint64_t> h_chain; DevMem<uint64_t> d_chain;
     // results live in MAPPED pinned host memory: the kernel stores sizes / digests straight over PCIe, so no small
     // device->host copies sit in a copy-engine queue behind multi-GiB frame copies
-    uint64_t *h_outlen = nullptr, *d_outlen = nullptr;  // same allocation, host / device view
-    uint8_t *h_md5 = nullptr, *d_md5 = nullptr;
-    cudaEvent_t ev_h2d = nullptr, ev_d2h = nullptr;  // input landed (on ctx->st_h2d) / frames landed (on ctx->st_d2h)
-    uint32_t *d_counters = nullptr;
-    uint8_t *d_scratch = nullptr;  // compress scratch: kScratchBytes per CTA of the grid (kernels of different slots overlap)
-    // receiver side
-    DecChunk *h_dchunks = nullptr, *d_dchunks = nullptr;
-    DecBlock *d_dblocks = nullptr;
-    uint32_t *d_blkdone = nullptr;
-    uint64_t dblocks_cap = 0;
-    int32_t *h_dstatus = nullptr, *d_dstatus = nullptr;  // pinned host mirror / device array
-    // E2EE (allocated when a key is set): box slab, per-chunk box descriptors, stream-block prefix, subkeys, nonces
-    uint8_t *d_box = nullptr;
-    BoxChunk *d_bchunks = nullptr;
-    uint64_t *d_blkbase = nullptr;
-    uint32_t *d_sub = nullptr;
-    uint8_t *h_nonce = nullptr, *d_nonce = nullptr;
-    uint64_t *h_boxmeta = nullptr, *d_boxmeta = nullptr;  // open side: box_off | box_len | frame_off (3 x n)
-    int32_t *h_bstatus = nullptr, *d_bstatus = nullptr;
-    uint32_t flags = 0;
-    // in-flight ticket
-    bool busy = false;
-    uint64_t ticket = 0;
-    uint32_t n = 0;
+    Mapped<uint64_t> outlen;
+    Mapped<uint8_t> md5;
+    DevMem<uint32_t> counters;
+    DevMem<uint8_t> scratch;  // compress scratch: kScratchBytes per CTA of the grid (kernels of different slots overlap)
+};
+struct DecodeArrays {  // receiver side
+    PinnedMem<DecChunk> h_chunks; DevMem<DecChunk> d_chunks;
+    PinnedMem<int32_t> h_status; DevMem<int32_t> d_status;
+    DevMem<uint32_t> d_dec_done;  // per chunk: leading blocks decoded (linked frames wait on it)
+    DevMem<DecBlock> d_blocks;    // per block of the batch: blocks_cap entries, grown on demand
+    DevMem<uint32_t> d_blk_done;
+    uint64_t blocks_cap = 0;
+};
+struct BoxArrays {  // E2EE: box slab, per-chunk box descriptors, stream-block prefix, subkeys, nonces, tag verdicts
+    DevMem<uint8_t> d_box;
+    PinnedMem<BoxChunk> h_chunks; DevMem<BoxChunk> d_chunks;  // (the host writes h_chunks and h_blk_base to open boxes)
+    PinnedMem<uint64_t> h_blk_base; DevMem<uint64_t> d_blk_base;
+    DevMem<uint32_t> d_sub;
+    PinnedMem<uint8_t> h_nonce; DevMem<uint8_t> d_nonce;
+    PinnedMem<int32_t> h_status; DevMem<int32_t> d_status;
+};
+struct Ticket {  // the batch a slot has in flight on the host path
+    bool busy = false, d2h_issued = false;
+    uint64_t id = 0;
+    uint32_t n = 0, flags = 0;
     std::vector<void *> dst;
     std::vector<uint64_t> out_off;
+};
+
+struct Slot {
+    Stream stream;
+    Event ev_k0, ev_k1;           // kernel_ms
+    Event ev_res;                 // kernel(s) done: sizes + digests are in host memory
+    Event ev_h2d, ev_d2h;         // input landed (on ctx->st_h2d) / frames landed (on ctx->st_d2h)
+    DevMem<uint8_t> d_in, d_out;  // host-path slabs (n_slots > 0)
+    BatchMeta meta;
+    DecodeArrays dec;
+    BoxArrays box;
+    Ticket ticket;
 };
 
 struct sky_ctx {
     int device = 0;
     int sm_count = 0;
-    uint64_t max_bytes = 0;
     uint32_t max_chunks = 0;
     uint64_t in_cap = 0, out_cap = 0;
-    std::vector<Slot> slots;  // slots[0] doubles as the metadata holder for sky_process_device
-    uint64_t next_ticket = 1;
-    uint64_t launches = 0;
-    std::string err;
     // Host path: every slot's input copies go FIFO through one H2D stream and every frame copy through one D2H
     // stream, so the two directions use different copy engines and batch k's frames leave while batch k+1's
     // input arrives (per-slot streams put both directions of all slots into one in-order engine queue).
-    cudaStream_t st_h2d = nullptr, st_d2h = nullptr;
-    uint8_t *d_key = nullptr;  // 32-byte SecretBox key (null: E2EE off)
-    bool trace = false;           // SKYCHUNK_TRACE=1: print per-batch device timeline to stderr
-    cudaEvent_t ev_base = nullptr;
+    Stream st_h2d, st_d2h;
+    std::vector<Slot> slots;  // slots[0] doubles as the metadata holder for sky_process_device
+    DevMem<uint8_t> d_key;    // 32-byte SecretBox key (null: E2EE off); set => every slot has its box arrays
+    uint64_t next_ticket = 1;
+    uint64_t launches = 0;
+    std::string err;
+    // The members release their resources after this body: first let every copy and kernel that may use them finish.
+    ~sky_ctx() {
+        if (st_h2d) cudaStreamSynchronize(st_h2d);
+        if (st_d2h) cudaStreamSynchronize(st_d2h);
+        for (Slot &s : slots)
+            if (s.stream) cudaStreamSynchronize(s.stream);
+    }
 };
 
 static thread_local std::string g_err;
@@ -716,6 +741,79 @@ static thread_local std::string g_err;
             return SKY_E_CUDA;                                                             \
         }                                                                                  \
     } while (0)
+
+static int build_slot(sky_ctx *ctx, Slot &s, bool slabs) {
+    const size_t nc = ctx->max_chunks, ng = (nc + 31) / 32 * 32;
+    CK(ctx, cudaStreamCreateWithFlags(s.stream.put(), cudaStreamNonBlocking));
+    CK(ctx, cudaEventCreate(s.ev_k0.put()));
+    CK(ctx, cudaEventCreate(s.ev_k1.put()));
+    CK(ctx, cudaEventCreate(s.ev_res.put()));
+    CK(ctx, cudaEventCreateWithFlags(s.ev_h2d.put(), cudaEventDisableTiming));
+    CK(ctx, cudaEventCreateWithFlags(s.ev_d2h.put(), cudaEventDisableTiming));
+    BatchMeta &m = s.meta;
+    CK(ctx, cudaMallocHost(m.h_desc.put(), nc * sizeof(ChunkDesc)));
+    CK(ctx, cudaMalloc(m.d_desc.put(), nc * sizeof(ChunkDesc)));
+    CK(ctx, cudaMallocHost(m.h_order.put(), ng * sizeof(uint32_t)));
+    CK(ctx, cudaMalloc(m.d_order.put(), ng * sizeof(uint32_t)));
+    CK(ctx, cudaMallocHost(m.h_chain.put(), nc * sizeof(uint64_t)));
+    CK(ctx, cudaMalloc(m.d_chain.put(), nc * sizeof(uint64_t)));
+    CK(ctx, m.outlen.alloc(nc));
+    CK(ctx, m.md5.alloc(nc * 16));
+    CK(ctx, cudaMalloc(m.counters.put(), 64));
+    CK(ctx, cudaMalloc(m.scratch.put(), (size_t)ctx->sm_count * kCtasPerSm * kScratchBytes));
+    if (slabs) {
+        cudaError_t e = cudaMalloc(s.d_in.put(), ctx->in_cap);
+        if (e == cudaSuccess) e = cudaMalloc(s.d_out.put(), ctx->out_cap);
+        if (e != cudaSuccess) { g_err = ctx->err = std::string("cudaMalloc(slab): ") + cudaGetErrorString(e); return SKY_E_NOMEM; }
+    }
+    return SKY_OK;
+}
+
+static int alloc_dec(sky_ctx *ctx, DecodeArrays &d) {
+    if (d.d_chunks) return SKY_OK;
+    const size_t nc = ctx->max_chunks;
+    DecodeArrays a;
+    CK(ctx, cudaMallocHost(a.h_chunks.put(), nc * sizeof(DecChunk)));
+    CK(ctx, cudaMalloc(a.d_chunks.put(), nc * sizeof(DecChunk)));
+    CK(ctx, cudaMallocHost(a.h_status.put(), nc * sizeof(int32_t)));
+    CK(ctx, cudaMalloc(a.d_status.put(), nc * sizeof(int32_t)));
+    CK(ctx, cudaMalloc(a.d_dec_done.put(), nc * sizeof(uint32_t)));
+    d = std::move(a);
+    return SKY_OK;
+}
+
+static int alloc_box(sky_ctx *ctx, BoxArrays &b) {
+    if (b.d_box) return SKY_OK;
+    const size_t nc = ctx->max_chunks;
+    BoxArrays a;
+    CK(ctx, cudaMalloc(a.d_box.put(), ctx->out_cap + 64 * nc + 256));
+    CK(ctx, cudaMallocHost(a.h_chunks.put(), nc * sizeof(BoxChunk)));
+    CK(ctx, cudaMalloc(a.d_chunks.put(), nc * sizeof(BoxChunk)));
+    CK(ctx, cudaMallocHost(a.h_blk_base.put(), (nc + 1) * sizeof(uint64_t)));
+    CK(ctx, cudaMalloc(a.d_blk_base.put(), (nc + 1) * sizeof(uint64_t)));
+    CK(ctx, cudaMalloc(a.d_sub.put(), nc * 16 * sizeof(uint32_t)));
+    CK(ctx, cudaMallocHost(a.h_nonce.put(), nc * 24));
+    CK(ctx, cudaMalloc(a.d_nonce.put(), nc * 24));
+    CK(ctx, cudaMallocHost(a.h_status.put(), nc * sizeof(int32_t)));
+    CK(ctx, cudaMalloc(a.d_status.put(), nc * sizeof(int32_t)));
+    b = std::move(a);
+    return SKY_OK;
+}
+
+// Block geometry of a batch (sender and receiver): visit(i, nblk) for every chunk, nblk = its number of 64 KiB blocks, and
+// rows = the largest nblk (at least 1): the persistent kernels take work item w = row * n + chunk from a 32-bit counter.
+// A chunk over kMaxChunkBlocks blocks, or a batch of 2^32 - 1 work items or more, is SKY_E_CAPACITY.
+template <class F>
+static int batch_geometry(uint32_t n, const uint64_t *len, uint32_t &rows, F &&visit) {
+    rows = 1;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint64_t nb = (len[i] + kBlock - 1) / kBlock;
+        if (nb > kMaxChunkBlocks) return SKY_E_CAPACITY;
+        visit(i, (uint32_t)nb);
+        rows = std::max(rows, (uint32_t)nb);
+    }
+    return (uint64_t)rows * n >= 0xffffffffull ? SKY_E_CAPACITY : SKY_OK;
+}
 
 extern "C" {
 
@@ -777,124 +875,43 @@ uint64_t sky_frame_bound(uint64_t n) {
 
 static uint64_t round16(uint64_t x) { return (x + 15) & ~15ull; }
 
-static int alloc_meta(sky_ctx *ctx, Slot &s, uint32_t max_chunks) {
-    const size_t nc = max_chunks, ng = (nc + 31) / 32 * 32;
-    CK(ctx, cudaMallocHost(&s.h_desc, nc * sizeof(ChunkDesc)));
-    CK(ctx, cudaMallocHost(&s.h_order, ng * sizeof(uint32_t)));
-    CK(ctx, cudaMallocHost(&s.h_chain, nc * sizeof(uint64_t)));
-    CK(ctx, cudaHostAlloc(&s.h_outlen, nc * sizeof(uint64_t), cudaHostAllocMapped | cudaHostAllocPortable));
-    CK(ctx, cudaHostAlloc(&s.h_md5, nc * 16, cudaHostAllocMapped | cudaHostAllocPortable));
-    CK(ctx, cudaHostGetDevicePointer(&s.d_outlen, s.h_outlen, 0));
-    CK(ctx, cudaHostGetDevicePointer(&s.d_md5, s.h_md5, 0));
-    CK(ctx, cudaEventCreateWithFlags(&s.ev_h2d, cudaEventDisableTiming));
-    CK(ctx, cudaEventCreateWithFlags(&s.ev_d2h, cudaEventDisableTiming));
-    CK(ctx, cudaMalloc(&s.d_desc, nc * sizeof(ChunkDesc)));
-    CK(ctx, cudaMalloc(&s.d_order, ng * sizeof(uint32_t)));
-    CK(ctx, cudaMalloc(&s.d_chain, nc * sizeof(uint64_t)));
-    CK(ctx, cudaMalloc(&s.d_counters, 64));
-    CK(ctx, cudaMalloc(&s.d_scratch, (size_t)ctx->sm_count * kCtasPerSm * kScratchBytes));
-    CK(ctx, cudaMallocHost(&s.h_dchunks, nc * sizeof(DecChunk)));
-    CK(ctx, cudaMalloc(&s.d_dchunks, nc * sizeof(DecChunk)));
-    CK(ctx, cudaMallocHost(&s.h_dstatus, nc * sizeof(int32_t)));
-    CK(ctx, cudaMalloc(&s.d_dstatus, nc * sizeof(int32_t)));
-    CK(ctx, cudaMalloc(&s.d_freed, nc * sizeof(uint32_t)));
-    CK(ctx, cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
-    CK(ctx, cudaEventCreate(&s.ev_k0));
-    CK(ctx, cudaEventCreate(&s.ev_k1));
-    CK(ctx, cudaEventCreate(&s.ev_res));
-    CK(ctx, cudaEventCreate(&s.ev_h0));
-    CK(ctx, cudaEventCreate(&s.ev_d0));
-    CK(ctx, cudaEventCreate(&s.ev_d1));
-    return SKY_OK;
-}
-
-static void free_slot(Slot &s) {
-    if (s.stream) cudaStreamSynchronize(s.stream);
-    cudaFreeHost(s.h_desc); cudaFreeHost(s.h_order); cudaFreeHost(s.h_chain); cudaFreeHost(s.h_outlen); cudaFreeHost(s.h_md5);
-    cudaFree(s.d_desc); cudaFree(s.d_order); cudaFree(s.d_chain); cudaFree(s.d_counters);
-    cudaFreeHost(s.h_dchunks); cudaFree(s.d_dchunks); cudaFree(s.d_dblocks); cudaFree(s.d_blkdone); cudaFreeHost(s.h_dstatus); cudaFree(s.d_dstatus); cudaFree(s.d_freed);
-    cudaFree(s.d_in); cudaFree(s.d_out); cudaFree(s.d_scratch);
-    cudaFree(s.d_box); cudaFree(s.d_bchunks); cudaFree(s.d_blkbase); cudaFree(s.d_sub); cudaFree(s.d_nonce); cudaFreeHost(s.h_nonce);
-    cudaFree(s.d_boxmeta); cudaFreeHost(s.h_boxmeta); cudaFree(s.d_bstatus); cudaFreeHost(s.h_bstatus);
-    if (s.ev_k0) cudaEventDestroy(s.ev_k0);
-    if (s.ev_k1) cudaEventDestroy(s.ev_k1);
-    if (s.ev_res) cudaEventDestroy(s.ev_res);
-    if (s.ev_h2d) cudaEventDestroy(s.ev_h2d);
-    if (s.ev_d2h) cudaEventDestroy(s.ev_d2h);
-    if (s.ev_h0) cudaEventDestroy(s.ev_h0);
-    if (s.ev_d0) cudaEventDestroy(s.ev_d0);
-    if (s.ev_d1) cudaEventDestroy(s.ev_d1);
-    if (s.stream) cudaStreamDestroy(s.stream);
-    s = Slot();
-}
-
 int sky_ctx_create(int device, uint64_t max_batch_bytes, uint32_t max_chunks, uint32_t n_slots, sky_ctx **out) {
     if (!out || max_chunks == 0) return SKY_E_INVALID;
     *out = nullptr;
     int ndev = 0;
     if (sky_device_count(&ndev) != SKY_OK) return SKY_E_NOGPU;
     if (device < 0 || device >= ndev) return SKY_E_INVALID;
-    sky_ctx *ctx = new (std::nothrow) sky_ctx();
+    std::unique_ptr<sky_ctx> ctx(new (std::nothrow) sky_ctx());  // an early return releases what was built so far
     if (!ctx) return SKY_E_NOMEM;
     ctx->device = device;
-    ctx->max_bytes = max_batch_bytes;
     ctx->max_chunks = max_chunks;
-    auto fail = [&](int rc) {
-        g_err = ctx->err;
-        for (auto &s : ctx->slots) free_slot(s);
-        if (ctx->st_h2d) cudaStreamDestroy(ctx->st_h2d);
-        if (ctx->st_d2h) cudaStreamDestroy(ctx->st_d2h);
-        delete ctx;
-        return rc;
-    };
-    cudaError_t e = cudaSetDevice(device);
-    if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return fail(SKY_E_CUDA); }
-    cudaDeviceProp prop;
-    e = cudaGetDeviceProperties(&prop, device);
-    if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return fail(SKY_E_CUDA); }
-    ctx->sm_count = prop.multiProcessorCount;
-    e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    if (e != cudaSuccess) {
-        ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (this build carries sm_90a code only)";
-        return fail(SKY_E_CUDA);
-    }
-    const uint32_t ns = n_slots ? n_slots : 1;
-    ctx->slots.resize(ns);
     // every chunk is placed at a 16-byte aligned offset; frames need bound(len) each
     ctx->in_cap = round16(max_batch_bytes) + 16ull * max_chunks + 256;
     ctx->out_cap = max_batch_bytes + (uint64_t)max_chunks * (64 + 4 * 2) + 4 * (max_batch_bytes / kBlock + 1) + 256;
-    for (uint32_t i = 0; i < ns; i++) {
-        int rc = alloc_meta(ctx, ctx->slots[i], max_chunks);
-        if (rc != SKY_OK) return fail(rc);
-        if (n_slots) {
-            e = cudaMalloc(&ctx->slots[i].d_in, ctx->in_cap);
-            if (e == cudaSuccess) e = cudaMalloc(&ctx->slots[i].d_out, ctx->out_cap);
-            if (e != cudaSuccess) { ctx->err = std::string("cudaMalloc(slab): ") + cudaGetErrorString(e); return fail(SKY_E_NOMEM); }
-        }
+    CK(ctx, cudaSetDevice(device));
+    CK(ctx, cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
+    cudaError_t e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (e != cudaSuccess) {
+        g_err = ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (this build carries sm_90a code only)";
+        return SKY_E_CUDA;
     }
     if (n_slots) {
-        e = cudaStreamCreateWithFlags(&ctx->st_h2d, cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->st_d2h, cudaStreamNonBlocking);
-        if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); return fail(SKY_E_CUDA); }
+        CK(ctx, cudaStreamCreateWithFlags(ctx->st_h2d.put(), cudaStreamNonBlocking));
+        CK(ctx, cudaStreamCreateWithFlags(ctx->st_d2h.put(), cudaStreamNonBlocking));
     }
-    ctx->trace = getenv("SKYCHUNK_TRACE") != nullptr;
-    if (ctx->trace) {
-        cudaEventCreate(&ctx->ev_base);
-        cudaEventRecord(ctx->ev_base, ctx->slots[0].stream);
+    ctx->slots.resize(n_slots ? n_slots : 1);
+    for (Slot &s : ctx->slots) {
+        const int rc = build_slot(ctx.get(), s, n_slots != 0);
+        if (rc != SKY_OK) return rc;
     }
-    *out = ctx;
+    *out = ctx.release();
     return SKY_OK;
 }
 
 int sky_ctx_destroy(sky_ctx *ctx) {
     if (!ctx) return SKY_E_INVALID;
     cudaSetDevice(ctx->device);
-    for (auto &s : ctx->slots) free_slot(s);
-    if (ctx->st_h2d) { cudaStreamSynchronize(ctx->st_h2d); cudaStreamDestroy(ctx->st_h2d); }
-    if (ctx->st_d2h) { cudaStreamSynchronize(ctx->st_d2h); cudaStreamDestroy(ctx->st_d2h); }
-    if (ctx->ev_base) cudaEventDestroy(ctx->ev_base);
-    cudaFree(ctx->d_key);
     delete ctx;
     return SKY_OK;
 }
@@ -915,51 +932,67 @@ int sky_pinned_free(void *p) {
 
 uint64_t sky_box_bound(uint64_t n) { return sky_frame_bound(n) + kBoxOverhead; }
 
-static int alloc_box(sky_ctx *ctx, Slot &s) {
-    if (s.d_box) return SKY_OK;
-    const size_t nc = ctx->max_chunks;
-    CK(ctx, cudaMalloc(&s.d_box, ctx->out_cap + 64 * nc + 256));
-    CK(ctx, cudaMalloc(&s.d_bchunks, nc * sizeof(BoxChunk)));
-    CK(ctx, cudaMalloc(&s.d_blkbase, (nc + 1) * sizeof(uint64_t)));
-    CK(ctx, cudaMalloc(&s.d_sub, nc * 16 * sizeof(uint32_t)));
-    CK(ctx, cudaMalloc(&s.d_nonce, nc * 24));
-    CK(ctx, cudaMallocHost(&s.h_nonce, nc * 24));
-    CK(ctx, cudaMalloc(&s.d_boxmeta, 3 * nc * sizeof(uint64_t)));
-    CK(ctx, cudaMallocHost(&s.h_boxmeta, 3 * nc * sizeof(uint64_t)));
-    CK(ctx, cudaMalloc(&s.d_bstatus, nc * sizeof(int32_t)));
-    CK(ctx, cudaMallocHost(&s.h_bstatus, nc * sizeof(int32_t)));
-    return SKY_OK;
-}
-
 int sky_set_e2ee_key(sky_ctx *ctx, const uint8_t *key32) {
     if (!ctx) return SKY_E_INVALID;
     CK(ctx, cudaSetDevice(ctx->device));
     if (!key32) {
-        cudaFree(ctx->d_key);
-        ctx->d_key = nullptr;
+        ctx->d_key.reset();
         return SKY_OK;
     }
-    if (!ctx->d_key) CK(ctx, cudaMalloc(&ctx->d_key, 32));
-    CK(ctx, cudaMemcpy(ctx->d_key, key32, 32, cudaMemcpyHostToDevice));
-    for (auto &s : ctx->slots) {
-        int rc = alloc_box(ctx, s);
+    for (Slot &s : ctx->slots) {  // boxes first: no key is installed unless every slot can seal and open
+        const int rc = alloc_box(ctx, s.box);
         if (rc != SKY_OK) return rc;
     }
+    DevMem<uint8_t> key;
+    CK(ctx, cudaMalloc(key.put(), 32));
+    CK(ctx, cudaMemcpy(key, key32, 32, cudaMemcpyHostToDevice));
+    ctx->d_key = std::move(key);  // (the previous key, if any, is released with `key`)
     return SKY_OK;
 }
 
 // Seal the batch's frames (or raw chunks) on `st` after the fused kernel: setup -> keys -> xor -> tag.
 static int launch_seal(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, uint8_t *d_dst, uint32_t flags) {
     const int use_frames = (flags & SKY_F_LZ4) ? 1 : 0;
-    sky_box_setup_kernel<<<1, 256, 0, st>>>(s.d_bchunks, s.d_blkbase, s.d_desc, n, s.d_outlen, d_dst, s.d_box, s.d_nonce, use_frames);
+    BoxArrays &b = s.box;
+    sky_box_setup_kernel<<<1, 256, 0, st>>>(b.d_chunks, b.d_blk_base, s.meta.d_desc, n, s.meta.outlen.d, d_dst, b.d_box, b.d_nonce, use_frames);
     CK(ctx, cudaGetLastError());
-    sky_box_keys_kernel<<<(n + 63) / 64, 64, 0, st>>>(s.d_bchunks, n, ctx->d_key, s.d_sub);
+    sky_box_keys_kernel<<<(n + 63) / 64, 64, 0, st>>>(b.d_chunks, n, ctx->d_key, b.d_sub);
     CK(ctx, cudaGetLastError());
-    sky_box_xor_kernel<<<ctx->sm_count * 8, 256, 0, st>>>(s.d_bchunks, s.d_blkbase, n, s.d_sub, 0);
+    sky_box_xor_kernel<<<ctx->sm_count * 8, 256, 0, st>>>(b.d_chunks, b.d_blk_base, n, b.d_sub, 0);
     CK(ctx, cudaGetLastError());
-    sky_box_tag_kernel<<<n, kPolyThreads, 0, st>>>(s.d_bchunks, s.d_sub, 0, nullptr);
+    sky_box_tag_kernel<<<n, kPolyThreads, 0, st>>>(b.d_chunks, b.d_sub, 0, nullptr);
     CK(ctx, cudaGetLastError());
     ctx->launches += 4;
+    return SKY_OK;
+}
+
+// Open the n boxes on slot `s`: copy box i to the box slab at frame_off[i] + 64 * i + 8, and open it into the frame slab at
+// frame_off[i] (msg_len[i] = its message bytes): keys -> tag -> xor, then the tag verdicts to the host.  Every offset and
+// length is known before the kernels run, so the host writes the descriptors.
+static int launch_open(sky_ctx *ctx, Slot &s, uint32_t n, const void *const *boxes, const uint64_t *box_len, const uint64_t *frame_off,
+                       uint64_t *msg_len) {
+    BoxArrays &b = s.box;
+    const cudaStream_t st = s.stream;
+    uint64_t acc = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        uint8_t *box = b.d_box + frame_off[i] + 64ull * i + 8;
+        CK(ctx, cudaMemcpyAsync(box, boxes[i], box_len[i], cudaMemcpyHostToDevice, st));
+        msg_len[i] = box_len[i] >= (uint64_t)kBoxOverhead ? box_len[i] - kBoxOverhead : 0;
+        b.h_chunks[i] = BoxChunk{box, s.d_out + frame_off[i], msg_len[i]};
+        b.h_blk_base[i] = acc;
+        acc += box_stream_blocks(msg_len[i]);
+    }
+    b.h_blk_base[n] = acc;
+    CK(ctx, cudaMemcpyAsync(b.d_chunks, b.h_chunks, n * sizeof(BoxChunk), cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemcpyAsync(b.d_blk_base, b.h_blk_base, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    sky_box_keys_kernel<<<(n + 63) / 64, 64, 0, st>>>(b.d_chunks, n, ctx->d_key, b.d_sub);
+    CK(ctx, cudaGetLastError());
+    sky_box_tag_kernel<<<n, kPolyThreads, 0, st>>>(b.d_chunks, b.d_sub, 1, b.d_status);
+    CK(ctx, cudaGetLastError());
+    sky_box_xor_kernel<<<ctx->sm_count * 8, 256, 0, st>>>(b.d_chunks, b.d_blk_base, n, b.d_sub, 1);
+    CK(ctx, cudaGetLastError());
+    CK(ctx, cudaMemcpyAsync(b.h_status, b.d_status, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    ctx->launches += 3;
     return SKY_OK;
 }
 
@@ -979,40 +1012,34 @@ static uint32_t fill_md5_order(uint32_t *order, uint32_t n, const uint64_t *len)
 static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t meta_st, uint32_t n, const uint8_t *d_src,
                         const uint64_t *src_off, const uint64_t *src_len, uint8_t *d_dst, const uint64_t *dst_off, uint32_t flags) {
     if ((flags & (SKY_F_LZ4 | SKY_F_MD5)) == 0) flags |= SKY_F_LZ4 | SKY_F_MD5;
-    uint32_t rows = 1;
-    for (uint32_t i = 0; i < n; i++) {
-        ChunkDesc &d = s.h_desc[i];
-        d.src = d_src + src_off[i];
-        d.dst = d_dst + dst_off[i];
-        d.len = src_len[i];
-        const uint64_t nb = (src_len[i] + kBlock - 1) / kBlock;
-        if (nb > kMaxChunkBlocks) return SKY_E_CAPACITY;
-        d.nblk = (uint32_t)nb;
-        rows = std::max(rows, d.nblk);
-        s.h_chain[i] = 15;  // block 0 starts right after the 15-byte frame header
-    }
-    if ((uint64_t)rows * n >= 0xffffffffull) return SKY_E_CAPACITY;
-    const uint32_t ng = fill_md5_order(s.h_order, n, src_len);
+    BatchMeta &m = s.meta;
+    uint32_t rows;
+    int rc = batch_geometry(n, src_len, rows, [&](uint32_t i, uint32_t nblk) {
+        m.h_desc[i] = ChunkDesc{d_src + src_off[i], d_dst + dst_off[i], src_len[i], nblk};
+        m.h_chain[i] = 15;  // block 0 starts right after the 15-byte frame header
+    });
+    if (rc != SKY_OK) return rc;
+    const uint32_t ng = fill_md5_order(m.h_order, n, src_len);
 
-    CK(ctx, cudaMemcpyAsync(s.d_desc, s.h_desc, n * sizeof(ChunkDesc), cudaMemcpyHostToDevice, meta_st));
-    CK(ctx, cudaMemcpyAsync(s.d_order, s.h_order, ng * 32 * sizeof(uint32_t), cudaMemcpyHostToDevice, meta_st));
-    CK(ctx, cudaMemcpyAsync(s.d_chain, s.h_chain, n * sizeof(uint64_t), cudaMemcpyHostToDevice, meta_st));
+    CK(ctx, cudaMemcpyAsync(m.d_desc, m.h_desc, n * sizeof(ChunkDesc), cudaMemcpyHostToDevice, meta_st));
+    CK(ctx, cudaMemcpyAsync(m.d_order, m.h_order, ng * 32 * sizeof(uint32_t), cudaMemcpyHostToDevice, meta_st));
+    CK(ctx, cudaMemcpyAsync(m.d_chain, m.h_chain, n * sizeof(uint64_t), cudaMemcpyHostToDevice, meta_st));
     if (meta_st != st) {
         CK(ctx, cudaEventRecord(s.ev_h2d, meta_st));  // input (enqueued earlier on meta_st) + metadata have landed
         CK(ctx, cudaStreamWaitEvent(st, s.ev_h2d, 0));
     }
-    CK(ctx, cudaMemsetAsync(s.d_counters, 0, 64, st));
-    memset(s.h_outlen, 0, n * sizeof(uint64_t));  // host-side clear (mapped memory; the slot is idle here)
-    memset(s.h_md5, 0, (size_t)n * 16);
+    CK(ctx, cudaMemsetAsync(m.counters, 0, 64, st));
+    memset(m.outlen.h, 0, n * sizeof(uint64_t));  // host-side clear (mapped memory; the slot is idle here)
+    memset(m.md5.h, 0, (size_t)n * 16);
 
     Params p;
-    p.chunks = s.d_desc;
-    p.md5_order = s.d_order;
-    p.chain = s.d_chain;
-    p.out_len = s.d_outlen;
-    p.md5_out = s.d_md5;
-    p.counters = s.d_counters;
-    p.scratch = s.d_scratch;
+    p.chunks = m.d_desc;
+    p.md5_order = m.d_order;
+    p.chain = m.d_chain;
+    p.out_len = m.outlen.d;
+    p.md5_out = m.md5.d;
+    p.counters = m.counters;
+    p.scratch = m.scratch;
     p.n_chunks = n;
     p.n_groups = ng;
     const uint32_t grid = (uint32_t)ctx->sm_count * kCtasPerSm;
@@ -1029,7 +1056,7 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
     CK(ctx, cudaEventRecord(s.ev_k1, st));
     ctx->launches++;
     if (flags & SKY_F_E2EE) {
-        int rc = launch_seal(ctx, s, st, n, d_dst, flags);
+        rc = launch_seal(ctx, s, st, n, d_dst, flags);
         if (rc != SKY_OK) return rc;
     }
     CK(ctx, cudaEventRecord(s.ev_res, st));  // kernel(s) done => sizes + digests are in host memory
@@ -1040,21 +1067,20 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
 // calls this: for each in-flight slot whose sizes have reached the host (ev_res done) it enqueues the exact-length
 // D2H copies on the ctx's D2H stream, so batch k's D2H overlaps batch k+1's H2D and kernel without a helper thread.
 static int issue_d2h(sky_ctx *ctx, Slot &s) {
+    Ticket &t = s.ticket;
     CK(ctx, cudaStreamWaitEvent(ctx->st_d2h, s.ev_res, 0));
-    if (ctx->trace) CK(ctx, cudaEventRecord(s.ev_d0, ctx->st_d2h));
-    for (uint32_t i = 0; i < s.n; i++) {
-        if (s.h_outlen[i] == 0) continue;  // MD5-only batch without E2EE: nothing comes back but the digests
-        const uint8_t *from = (s.flags & SKY_F_E2EE) ? s.d_box + s.out_off[i] + 64ull * i + 8 : s.d_out + s.out_off[i];
-        CK(ctx, cudaMemcpyAsync(s.dst[i], from, s.h_outlen[i], cudaMemcpyDeviceToHost, ctx->st_d2h));
+    for (uint32_t i = 0; i < t.n; i++) {
+        if (s.meta.outlen.h[i] == 0) continue;  // MD5-only batch without E2EE: nothing comes back but the digests
+        const uint8_t *from = (t.flags & SKY_F_E2EE) ? s.box.d_box + t.out_off[i] + 64ull * i + 8 : s.d_out + t.out_off[i];
+        CK(ctx, cudaMemcpyAsync(t.dst[i], from, s.meta.outlen.h[i], cudaMemcpyDeviceToHost, ctx->st_d2h));
     }
-    if (ctx->trace) CK(ctx, cudaEventRecord(s.ev_d1, ctx->st_d2h));
     CK(ctx, cudaEventRecord(s.ev_d2h, ctx->st_d2h));
-    s.d2h_issued = true;
+    t.d2h_issued = true;
     return SKY_OK;
 }
 static int progress(sky_ctx *ctx) {
-    for (auto &s : ctx->slots) {
-        if (!s.busy || s.d2h_issued) continue;
+    for (Slot &s : ctx->slots) {
+        if (!s.ticket.busy || s.ticket.d2h_issued) continue;
         cudaError_t q = cudaEventQuery(s.ev_res);
         if (q == cudaErrorNotReady) continue;
         CK(ctx, q);
@@ -1078,13 +1104,13 @@ int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64
     }
     CK(ctx, cudaSetDevice(ctx->device));
     Slot &s = ctx->slots[0];
-    if (s.busy) return SKY_E_BUSY;
+    if (s.ticket.busy) return SKY_E_BUSY;
     cudaStream_t st = stream ? (cudaStream_t)stream : s.stream;
     int rc = launch_batch(ctx, s, st, st, n, (const uint8_t *)d_src, src_off, src_len, (uint8_t *)d_dst, dst_off, flags);
     if (rc != SKY_OK) return rc;
     CK(ctx, cudaStreamSynchronize(st));
-    if (out_len) memcpy(out_len, s.h_outlen, n * sizeof(uint64_t));
-    if (md5) memcpy(md5, s.h_md5, (size_t)n * 16);
+    if (out_len) memcpy(out_len, s.meta.outlen.h, n * sizeof(uint64_t));
+    if (md5) memcpy(md5, s.meta.md5.h, (size_t)n * 16);
     if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, s.ev_k0, s.ev_k1));
     return SKY_OK;
 }
@@ -1099,8 +1125,8 @@ int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t 
     if (e2ee && (!ctx->d_key || !nonces)) return SKY_E_NOKEY;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
     Slot *sp = nullptr;
-    for (auto &s : ctx->slots)
-        if (!s.busy && s.d_in) { sp = &s; break; }
+    for (Slot &s : ctx->slots)
+        if (!s.ticket.busy && s.d_in) { sp = &s; break; }
     if (!sp) return ctx->slots[0].d_in ? SKY_E_BUSY : SKY_E_INVALID;
     Slot &s = *sp;
     CK(ctx, cudaSetDevice(ctx->device));
@@ -1119,57 +1145,40 @@ int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t 
         op += round16(sky_frame_bound(src_len[i]));
     }
     if (ip > ctx->in_cap || op > ctx->out_cap) return SKY_E_CAPACITY;
-    if (ctx->trace) CK(ctx, cudaEventRecord(s.ev_h0, ctx->st_h2d));
     for (uint32_t i = 0; i < n; i++)
         if (src_len[i]) CK(ctx, cudaMemcpyAsync(s.d_in + in_off[i], src[i], src_len[i], cudaMemcpyHostToDevice, ctx->st_h2d));
     if (e2ee) {
-        memcpy(s.h_nonce, nonces, 24ull * n);
-        CK(ctx, cudaMemcpyAsync(s.d_nonce, s.h_nonce, 24ull * n, cudaMemcpyHostToDevice, ctx->st_h2d));
+        memcpy(s.box.h_nonce, nonces, 24ull * n);
+        CK(ctx, cudaMemcpyAsync(s.box.d_nonce, s.box.h_nonce, 24ull * n, cudaMemcpyHostToDevice, ctx->st_h2d));
     }
-    s.flags = flags;
     int rc = launch_batch(ctx, s, s.stream, ctx->st_h2d, n, s.d_in, in_off.data(), src_len, s.d_out, out_off.data(), flags);
     if (rc != SKY_OK) return rc;
-    s.busy = true;
-    s.d2h_issued = false;
-    s.ticket = ctx->next_ticket++;
-    s.n = n;
-    if (returns_data) s.dst.assign(dst, dst + n); else s.dst.assign(n, nullptr);
-    s.out_off.swap(out_off);
-    *ticket = s.ticket;
+    s.ticket = Ticket{true, false, ctx->next_ticket++, n, flags,
+                      returns_data ? std::vector<void *>(dst, dst + n) : std::vector<void *>(n), std::move(out_off)};
+    *ticket = s.ticket.id;
     return SKY_OK;
 }
 
 int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
     if (!ctx) return SKY_E_INVALID;
     Slot *sp = nullptr;
-    for (auto &s : ctx->slots)
-        if (s.busy && s.ticket == ticket) { sp = &s; break; }
+    for (Slot &s : ctx->slots)
+        if (s.ticket.busy && s.ticket.id == ticket) { sp = &s; break; }
     if (!sp) return SKY_E_TICKET;
     Slot &s = *sp;
     CK(ctx, cudaSetDevice(ctx->device));
     { int prc = progress(ctx); if (prc != SKY_OK) return prc; }
-    if (!s.d2h_issued) {
+    if (!s.ticket.d2h_issued) {
         CK(ctx, cudaEventSynchronize(s.ev_res));  // sizes + digests are on the host now
         int rc = issue_d2h(ctx, s);
         if (rc != SKY_OK) return rc;
     }
     { int prc = progress(ctx); if (prc != SKY_OK) return prc; }  // let later batches' copies queue up behind ours
     CK(ctx, cudaEventSynchronize(s.ev_d2h));
-    if (out_len) memcpy(out_len, s.h_outlen, s.n * sizeof(uint64_t));
-    if (md5) memcpy(md5, s.h_md5, (size_t)s.n * 16);
+    if (out_len) memcpy(out_len, s.meta.outlen.h, s.ticket.n * sizeof(uint64_t));
+    if (md5) memcpy(md5, s.meta.md5.h, (size_t)s.ticket.n * 16);
     if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, s.ev_k0, s.ev_k1));
-    if (ctx->trace) {
-        float h0 = 0, k0 = 0, k1 = 0, rs = 0, d0 = 0, d1 = 0;
-        cudaEventElapsedTime(&h0, ctx->ev_base, s.ev_h0);
-        cudaEventElapsedTime(&k0, ctx->ev_base, s.ev_k0);
-        cudaEventElapsedTime(&k1, ctx->ev_base, s.ev_k1);
-        cudaEventElapsedTime(&rs, ctx->ev_base, s.ev_res);
-        cudaEventElapsedTime(&d0, ctx->ev_base, s.ev_d0);
-        cudaEventElapsedTime(&d1, ctx->ev_base, s.ev_d1);
-        fprintf(stderr, "[skychunk trace] ticket %llu: h2d %.1f..%.1f kernel %.1f..%.1f results %.1f d2h %.1f..%.1f ms\n",
-                (unsigned long long)s.ticket, h0, k0, k0, k1, rs, d0, d1);
-    }
-    s.busy = false;
+    s.ticket.busy = false;
     return SKY_OK;
 }
 
@@ -1204,62 +1213,52 @@ int sky_memcpy_d2h(sky_ctx *ctx, void *host, const void *dptr, uint64_t bytes) {
 // Enqueues index + decode (+ MD5 of the decoded bytes through the fused kernel's MD5 role) on `st`.
 static int launch_decode(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, const uint8_t *d_frames, const uint64_t *frame_off,
                          const uint64_t *frame_len, uint8_t *d_out, const uint64_t *out_off, const uint64_t *raw_len) {
+    int rc = alloc_dec(ctx, s.dec);
+    if (rc != SKY_OK) return rc;
+    DecodeArrays &d = s.dec;
     uint64_t nblk_total = 0;
-    uint32_t rows = 1;
-    for (uint32_t i = 0; i < n; i++) {
-        DecChunk &d = s.h_dchunks[i];
-        d.frame = d_frames + frame_off[i];
-        d.out = d_out + out_off[i];
-        d.frame_len = frame_len[i];
-        d.raw_len = raw_len[i];
-        const uint64_t nb = (raw_len[i] + kBlock - 1) / kBlock;
-        if (nb > kMaxChunkBlocks) return SKY_E_CAPACITY;
-        d.nblk = (uint32_t)nb;
-        d.blk_base = nblk_total;
-        d.linked = 0;
-        nblk_total += nb;
-        rows = std::max(rows, d.nblk);
+    uint32_t rows;
+    rc = batch_geometry(n, raw_len, rows, [&](uint32_t i, uint32_t nblk) {
+        d.h_chunks[i] = DecChunk{d_frames + frame_off[i], d_out + out_off[i], frame_len[i], raw_len[i], nblk_total, nblk, 0};
+        nblk_total += nblk;
+    });
+    if (rc != SKY_OK) return rc;
+    if (nblk_total + 1 > d.blocks_cap) {
+        CK(ctx, cudaStreamSynchronize(st));  // the previous decode is done with the old arrays
+        d.blocks_cap = 0;
+        CK(ctx, cudaMalloc(d.d_blocks.put(), (nblk_total + 1) * sizeof(DecBlock)));
+        CK(ctx, cudaMalloc(d.d_blk_done.put(), (nblk_total + 1) * sizeof(uint32_t)));
+        d.blocks_cap = nblk_total + 1;
     }
-    if ((uint64_t)rows * n >= 0xffffffffull) return SKY_E_CAPACITY;
-    if (nblk_total + 1 > s.dblocks_cap) {
-        CK(ctx, cudaStreamSynchronize(st));
-        cudaFree(s.d_dblocks);
-        cudaFree(s.d_blkdone);
-        s.d_dblocks = nullptr;
-        s.d_blkdone = nullptr;
-        s.dblocks_cap = 0;
-        CK(ctx, cudaMalloc(&s.d_dblocks, (nblk_total + 1) * sizeof(DecBlock)));
-        CK(ctx, cudaMalloc(&s.d_blkdone, (nblk_total + 1) * sizeof(uint32_t)));
-        s.dblocks_cap = nblk_total + 1;
-    }
-    CK(ctx, cudaMemcpyAsync(s.d_dchunks, s.h_dchunks, n * sizeof(DecChunk), cudaMemcpyHostToDevice, st));
-    CK(ctx, cudaMemsetAsync(s.d_counters, 0, 64, st));
-    CK(ctx, cudaMemsetAsync(s.d_freed, 0, n * sizeof(uint32_t), st));
-    CK(ctx, cudaMemsetAsync(s.d_dstatus, 0, n * sizeof(int32_t), st));
-    CK(ctx, cudaMemsetAsync(s.d_blkdone, 0, (nblk_total + 1) * sizeof(uint32_t), st));
-    const uint32_t ng = fill_md5_order(s.h_order, n, raw_len);
-    CK(ctx, cudaMemcpyAsync(s.d_order, s.h_order, ng * 32 * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-    memset(s.h_md5, 0, (size_t)n * 16);
+    BatchMeta &m = s.meta;
+    CK(ctx, cudaMemcpyAsync(d.d_chunks, d.h_chunks, n * sizeof(DecChunk), cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemsetAsync(m.counters, 0, 64, st));
+    CK(ctx, cudaMemsetAsync(d.d_dec_done, 0, n * sizeof(uint32_t), st));
+    CK(ctx, cudaMemsetAsync(d.d_status, 0, n * sizeof(int32_t), st));
+    CK(ctx, cudaMemsetAsync(d.d_blk_done, 0, (nblk_total + 1) * sizeof(uint32_t), st));
+    const uint32_t ng = fill_md5_order(m.h_order, n, raw_len);
+    CK(ctx, cudaMemcpyAsync(m.d_order, m.h_order, ng * 32 * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    memset(m.md5.h, 0, (size_t)n * 16);
     DecParams p;
-    p.chunks = s.d_dchunks;
-    p.blocks = s.d_dblocks;
-    p.status = s.d_dstatus;
-    p.done = s.d_freed;
-    p.counter = s.d_counters;
-    p.blk_done = s.d_blkdone;
-    p.md5_order = s.d_order;
-    p.md5_out = s.d_md5;
+    p.chunks = d.d_chunks;
+    p.blocks = d.d_blocks;
+    p.status = d.d_status;
+    p.dec_done = d.d_dec_done;
+    p.counter = m.counters;
+    p.blk_done = d.d_blk_done;
+    p.md5_order = m.d_order;
+    p.md5_out = m.md5.d;
     p.n_chunks = n;
     p.n_groups = ng;
     p.rows = rows;
-    CK(ctx, cudaEventRecord(s.ev_h0, st));  // start marker of the receiver-side kernels
+    CK(ctx, cudaEventRecord(s.ev_k0, st));
     sky_frame_index_kernel<<<(n + 127) / 128, 128, 0, st>>>(p);
     CK(ctx, cudaGetLastError());
     sky_decode_kernel<<<ctx->sm_count, 512, kMd5WarpsPerCta * kRingBytes, st>>>(p);
     CK(ctx, cudaGetLastError());
     CK(ctx, cudaEventRecord(s.ev_k1, st));
     ctx->launches += 2;
-    CK(ctx, cudaMemcpyAsync(s.h_dstatus, s.d_dstatus, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CK(ctx, cudaMemcpyAsync(d.h_status, d.d_status, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     return SKY_OK;
 }
 
@@ -1275,14 +1274,14 @@ int sky_decode_device(sky_ctx *ctx, uint32_t n, const void *d_frames, const uint
     }
     CK(ctx, cudaSetDevice(ctx->device));
     Slot &s = ctx->slots[0];
-    if (s.busy) return SKY_E_BUSY;
+    if (s.ticket.busy) return SKY_E_BUSY;
     cudaStream_t st = stream ? (cudaStream_t)stream : s.stream;
     int rc = launch_decode(ctx, s, st, n, (const uint8_t *)d_frames, frame_off, frame_len, (uint8_t *)d_out, out_off, raw_len);
     if (rc != SKY_OK) return rc;
     CK(ctx, cudaStreamSynchronize(st));
-    if (status) memcpy(status, s.h_dstatus, n * sizeof(int32_t));
-    if (md5) memcpy(md5, s.h_md5, (size_t)n * 16);
-    if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, s.ev_h0, s.ev_k1));  // index + decode + MD5
+    if (status) memcpy(status, s.dec.h_status, n * sizeof(int32_t));
+    if (md5) memcpy(md5, s.meta.md5.h, (size_t)n * 16);
+    if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, s.ev_k0, s.ev_k1));  // index + decode + MD5
     return SKY_OK;
 }
 
@@ -1291,7 +1290,7 @@ int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64
     if (!ctx || n == 0 || !frames || !frame_len || !dst || !raw_len) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
     Slot &s = ctx->slots[0];
-    if (s.busy) return SKY_E_BUSY;
+    if (s.ticket.busy) return SKY_E_BUSY;
     if (!s.d_in) return SKY_E_INVALID;  // ctx created without slabs
     const bool e2ee = (flags & SKY_F_E2EE) != 0;
     if (e2ee && !ctx->d_key) return SKY_E_NOKEY;
@@ -1309,26 +1308,8 @@ int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64
     if (fp > ctx->out_cap || op > ctx->in_cap) return SKY_E_CAPACITY;
     if (e2ee) {
         // the payloads are boxes (nonce | tag | ciphertext): check the tags, decrypt into the frame slab, then decode as usual
-        int rc = alloc_box(ctx, s);
+        int rc = launch_open(ctx, s, n, frames, frame_len, f_off.data(), f_len.data());
         if (rc != SKY_OK) return rc;
-        for (uint32_t i = 0; i < n; i++) {
-            s.h_boxmeta[i] = f_off[i] + 64ull * i;
-            s.h_boxmeta[n + i] = frame_len[i];
-            s.h_boxmeta[2 * n + i] = f_off[i];
-            CK(ctx, cudaMemcpyAsync(s.d_box + f_off[i] + 64ull * i + 8, frames[i], frame_len[i], cudaMemcpyHostToDevice, s.stream));
-            f_len[i] = frame_len[i] >= (uint64_t)kBoxOverhead ? frame_len[i] - kBoxOverhead : 0;
-        }
-        CK(ctx, cudaMemcpyAsync(s.d_boxmeta, s.h_boxmeta, 3ull * n * sizeof(uint64_t), cudaMemcpyHostToDevice, s.stream));
-        sky_box_open_setup_kernel<<<1, 256, 0, s.stream>>>(s.d_bchunks, s.d_blkbase, n, s.d_boxmeta, s.d_boxmeta + n, s.d_boxmeta + 2 * n, s.d_out, s.d_box);
-        CK(ctx, cudaGetLastError());
-        sky_box_keys_kernel<<<(n + 63) / 64, 64, 0, s.stream>>>(s.d_bchunks, n, ctx->d_key, s.d_sub);
-        CK(ctx, cudaGetLastError());
-        sky_box_tag_kernel<<<n, kPolyThreads, 0, s.stream>>>(s.d_bchunks, s.d_sub, 1, s.d_bstatus);
-        CK(ctx, cudaGetLastError());
-        sky_box_xor_kernel<<<ctx->sm_count * 8, 256, 0, s.stream>>>(s.d_bchunks, s.d_blkbase, n, s.d_sub, 1);
-        CK(ctx, cudaGetLastError());
-        CK(ctx, cudaMemcpyAsync(s.h_bstatus, s.d_bstatus, n * sizeof(int32_t), cudaMemcpyDeviceToHost, s.stream));
-        ctx->launches += 4;
     } else {
         for (uint32_t i = 0; i < n; i++)
             CK(ctx, cudaMemcpyAsync(s.d_out + f_off[i], frames[i], frame_len[i], cudaMemcpyHostToDevice, s.stream));
@@ -1337,13 +1318,13 @@ int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64
     if (rc != SKY_OK) return rc;
     if (e2ee) {
         for (uint32_t i = 0; i < n; i++)
-            if (s.h_bstatus[i] != 0 || frame_len[i] < (uint64_t)kBoxOverhead) {  // forged or truncated box: never hand its bytes out
-                s.h_dstatus[i] = SKY_D_AUTH;
+            if (s.box.h_status[i] != 0 || frame_len[i] < (uint64_t)kBoxOverhead) {  // forged or truncated box: never hand its bytes out
+                s.dec.h_status[i] = SKY_D_AUTH;
                 if (status) status[i] = SKY_D_AUTH;
             }
     }
     for (uint32_t i = 0; i < n; i++)
-        if (raw_len[i] && s.h_dstatus[i] == 0)
+        if (raw_len[i] && s.dec.h_status[i] == 0)
             CK(ctx, cudaMemcpyAsync(dst[i], s.d_in + o_off[i], raw_len[i], cudaMemcpyDeviceToHost, s.stream));
     CK(ctx, cudaStreamSynchronize(s.stream));
     return SKY_OK;
