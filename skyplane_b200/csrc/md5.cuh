@@ -2,9 +2,10 @@
 //
 // Replaces hashlib.md5().update()/digest() at skyplane/obj_store/s3_interface.py:181-192.
 // One chunk is ONE serial chain (the digest must equal hashlib.md5(whole chunk)), so a warp
-// carries 32 chunks, lane = chunk.  The per-step dependent chain is 3 SASS ops:
-//   LOP3 (F/G/H/I of the newest b) -> IADD3 (+ a + M[g] + K[i], pre-added off the chain)
+// carries 32 chunks, lane = chunk.  The per-step dependent chain is 3 SASS ops, all on the ALU pipe:
+//   LOP3 (F/G/H/I of the newest b) -> IADD3 (+ (a + M[g]) + K[i]; a + M[g] is an IMAD on the FMA pipe, off the chain)
 //   -> LEA.HI (b + rotl(t, s): ptxas fuses the funnel shift and the add).
+// Each ALU -> ALU hop is 4 cycles, so a step is scheduled at 12 (tools/md5_schedule.py reads it from the SASS).
 // Message words are staged into shared memory with 16-byte cp.async SKY_MD5_SLOTS-1 blocks ahead of the
 // chain (ring of SKY_MD5_SLOTS x 64 B per lane, laid out [slot][piece][lane] so LDS.128 is conflict-free).
 #pragma once
@@ -30,27 +31,37 @@ __device__ __forceinline__ void md5_init(Md5State &s) {
     s.d = 0x10325476u;
 }
 
-// M[g] + K[i] is formed by an opaque add so ptxas cannot re-associate the constant onto the
-// dependent chain (it otherwise emits LOP3 -> IADD3 -> VIADD(+K) -> LEA.HI: four ops per step).
-__device__ __forceinline__ uint32_t md5_mk(uint32_t m, uint32_t k) {
+// a + M[g] is formed as M[g] * one + a, where `one` is 1 but ptxas cannot prove it (md5_one), so it stays an IMAD
+// on the FMA pipe, off the chain.  The on-chain add F + (a + M[g]) + K[i] is then one IADD3 with an immediate, which
+// has no IMAD form.  With a plain add ptxas forms a + M[g] + K[i] as the off-chain IADD3 and moves the on-chain add
+// to the FMA pipe as IMAD.IADD, and each hop between the pipes costs 5 cycles instead of 4 (14 cycles per step).
+__device__ __forceinline__ uint32_t md5_am(uint32_t a, uint32_t m, uint32_t one) {
     uint32_t r;
-    asm("add.u32 %0, %1, %2;" : "=r"(r) : "r"(m), "r"(k));
+    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(m), "r"(one), "r"(a));
     return r;
 }
-#define SKY_MD5_STEP(FN, a, b, c, d, m, k, s)                 \
-    {                                                         \
-        uint32_t t_ = a + md5_mk((m), (k)) + FN(b, c, d);     \
-        a = b + __funnelshift_l(t_, t_, s);                   \
+// 1, read from special registers: the only bit set in %lanemask_eq is bit %laneid.
+__device__ __forceinline__ uint32_t md5_one() {
+    uint32_t eq, lane;
+    asm("mov.u32 %0, %%lanemask_eq;" : "=r"(eq));
+    asm("mov.u32 %0, %%laneid;" : "=r"(lane));
+    return eq >> lane;
+}
+#define SKY_MD5_STEP(FN, a, b, c, d, m, k, s)                      \
+    {                                                              \
+        uint32_t t_ = FN(b, c, d) + md5_am(a, (m), one) + (k);     \
+        a = b + __funnelshift_l(t_, t_, s);                        \
     }
 #define SKY_F(b, c, d) ((d) ^ ((b) & ((c) ^ (d))))
 #define SKY_G(b, c, d) ((c) ^ ((d) & ((b) ^ (c))))
 #define SKY_H(b, c, d) ((b) ^ (c) ^ (d))
 #define SKY_I(b, c, d) ((c) ^ ((b) | ~(d)))
 
-// Round R (16 steps) of one 64-byte block on the working state; w[16] = little-endian message words.  md5_warp
-// interleaves its staging between the rounds, so they are separate functions.
+// Round R (16 steps) of one 64-byte block on the working state; w[16] = little-endian message words, one = md5_one().
+// md5_warp interleaves its staging between the rounds, so they are separate functions.
 template <int R>
-__device__ __forceinline__ void md5_round(uint32_t &a, uint32_t &b, uint32_t &c, uint32_t &d, const uint32_t (&w)[16]) {
+__device__ __forceinline__ void md5_round(uint32_t &a, uint32_t &b, uint32_t &c, uint32_t &d, const uint32_t (&w)[16],
+                                          uint32_t one) {
     if constexpr (R == 0) {
         SKY_MD5_STEP(SKY_F, a, b, c, d, w[0], 0xd76aa478, 7)
         SKY_MD5_STEP(SKY_F, d, a, b, c, w[1], 0xe8c7b756, 12)
@@ -123,12 +134,12 @@ __device__ __forceinline__ void md5_round(uint32_t &a, uint32_t &b, uint32_t &c,
 }
 
 // One 64-byte block.
-__device__ __forceinline__ void md5_block(Md5State &st, const uint32_t (&w)[16]) {
+__device__ __forceinline__ void md5_block(Md5State &st, const uint32_t (&w)[16], uint32_t one) {
     uint32_t a = st.a, b = st.b, c = st.c, d = st.d;
-    md5_round<0>(a, b, c, d, w);
-    md5_round<1>(a, b, c, d, w);
-    md5_round<2>(a, b, c, d, w);
-    md5_round<3>(a, b, c, d, w);
+    md5_round<0>(a, b, c, d, w, one);
+    md5_round<1>(a, b, c, d, w, one);
+    md5_round<2>(a, b, c, d, w, one);
+    md5_round<3>(a, b, c, d, w, one);
     st.a += a;
     st.b += b;
     st.c += c;
@@ -194,6 +205,7 @@ __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uin
     // slot s, piece q of this lane lives at ring[((s*4 + q)*32 + lane) * 4 words]: a per-lane base plus an immediate
     const uint32_t *lring = ring + lane * 4;
     const uint32_t lring_s = (uint32_t)__cvta_generic_to_shared(lring);
+    const uint32_t one = md5_one();
 
     gate(0, active && len > 0);
     md5_unroll<kSlots - 1>([&](auto sc) {
@@ -226,14 +238,14 @@ __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uin
             constexpr int ps = (u + kSlots - 1) & (kSlots - 1);  // slot of block i+u-1, read during block i+u-2
             constexpr int ns = (u + 1) & (kSlots - 1);
             uint32_t a = st.a, b = st.b, c = st.c, d = st.d;
-            md5_round<0>(a, b, c, d, w[u & 1]);
+            md5_round<0>(a, b, c, d, w[u & 1], one);
             cp_async_block<ps>(i + u + (kSlots - 1) < nfull, lring_s, pf_src + u * 64);
-            md5_round<1>(a, b, c, d, w[u & 1]);
+            md5_round<1>(a, b, c, d, w[u & 1], one);
             cp_async_commit();
             cp_async_wait<kSlots - 2>();  // block i+u+1 has landed
-            md5_round<2>(a, b, c, d, w[u & 1]);
+            md5_round<2>(a, b, c, d, w[u & 1], one);
             load_words(w[(u + 1) & 1], ns);
-            md5_round<3>(a, b, c, d, w[u & 1]);
+            md5_round<3>(a, b, c, d, w[u & 1], one);
             st.a += a;
             st.b += b;
             st.c += c;
@@ -274,7 +286,7 @@ __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uin
             uint32_t w[16];
 #pragma unroll
             for (int k = 0; k < 16; k++) w[k] = tw[16 * t + k];
-            md5_block(st, w);
+            md5_block(st, w, one);
         }
         uint4 dg = make_uint4(st.a, st.b, st.c, st.d);
         *reinterpret_cast<uint4 *>(out) = dg;  // out is 16-byte aligned (md5 array base is 256-aligned)

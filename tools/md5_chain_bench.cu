@@ -1,6 +1,6 @@
 // md5_chain_bench.cu -- measures the dependent-chain latency of one MD5 block per lane on sm_90a
-// for several instruction selections of the on-chain add.  Not product code: a measurement tool whose
-// result picks the formulation used in skyplane_b200/csrc/md5.cuh.
+// for several instruction selections of the on-chain add.  Not product code: a measurement tool.  (md5.cuh's own
+// selection -- a + M[g] as an IMAD off the chain, an all-ALU chain -- is measured by the in-situ mode below.)
 //   V0: plain C (ptxas picks IMAD.IADD for the on-chain add: alu -> fma -> alu)
 //   V1: on-chain add forced onto the ALU pipe by consuming its carry (IADD3 with carry-out)
 //   V2: 3-input on-chain add (a, m+K, f) kept separate via carry trick on the inner add
