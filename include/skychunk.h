@@ -57,6 +57,11 @@ extern "C" {
  * e2ee_key_bytes (gateway_operator.py:183-186, :362-364) and the receiver undoes (gateway_receiver.py:191-193). */
 #define SKY_F_E2EE 16u
 #define SKY_BOX_OVERHEAD 40u
+/* high-ratio frames (sky_submit, with or without SKY_F_E2EE, and sky_process_device): the same frame format, made by a
+ * hash-chain match search with a lazy parse instead of the fast single-candidate parse.  Alone it means
+ * LZ4 + MD5 + HC, as 0 means LZ4 + MD5; with stage bits it needs SKY_F_LZ4 (SKY_F_MD5 | SKY_F_HC is SKY_E_INVALID).
+ * The digests come from the fused kernel's MD5-only mode running beside the HC kernel (two launches per batch). */
+#define SKY_F_HC 32u
 
 typedef struct sky_ctx sky_ctx;
 
@@ -68,8 +73,10 @@ SKY_API int sky_device_count(int *count);
  * unlike nvidia-smi -i); the host side maps it to the GPU's NUMA node before pinning staging memory. */
 SKY_API int sky_device_pci_bus_id(int device, char *buf, int len);
 /* Compile-time constants of the kernels in this build (tuning builds differ): what = 0 -> LZ4 match-table entries per
- * CTA, 1 -> warps per CTA of the fused kernel, 2 -> probe slots per segment, 3 -> log2 of the largest probe stride.
- * Unknown `what` returns 0.  Parity tests feed these to the sequential twin of the compressor (tools/lz4_tile_model.c). */
+ * CTA, 1 -> warps per CTA of the fused kernel, 2 -> probe slots per segment, 3 -> log2 of the largest probe stride;
+ * SKY_F_HC: 4 -> chain candidates searched per position, 5 -> log2 of the hash-head entries, 6 -> length at which a
+ * position's search stops.  Unknown `what` returns 0 (so a library without SKY_F_HC reads 0 for 4..6).  Parity tests feed
+ * these to the sequential twins of the compressors (tools/lz4_tile_model.c, tools/lz4hc_model.c). */
 SKY_API uint32_t sky_kernel_config(int what);
 
 /* Worst-case frame bytes for an n-byte chunk: 15 + n + 4*ceil(n/65536) + 4 (11 when n == 0). */

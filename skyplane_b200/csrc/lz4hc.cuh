@@ -1,0 +1,218 @@
+// lz4hc.cuh -- high-ratio LZ4 block compressor for sm_90a (SKY_F_HC): exact hash chains, a bounded search per position
+// and a lazy parse, in the same frame layout as the fast compressor (independent 64 KiB blocks, stored-raw fallback).
+//
+// tools/lz4hc_model.c is the sequential twin: it states the chain rule, candidate order, tie rule, lazy rule and emission,
+// and the frames of this kernel are byte-identical to it (tests/test_gpu_hc.py).  One CTA owns one 64 KiB block at a time,
+// claimed row-major from the batch's work counter (claim_block), in five steps:
+//   load   : one bulk async copy of the block into shared memory (the head table is cleared meanwhile);
+//   chains : warp 0 inserts the positions 32 at a time.  A lane's predecessor is the highest lower lane with its hash
+//            (match.any), else head[hash]; then the highest lane of each hash writes head.  That is sequential insertion.
+//            chain[p] is the distance to p's predecessor (u16, 0 = none), head[h] the latest position + 1 (u16, 0 = none);
+//   search : every thread takes positions tid, tid + 1024, ...: walk at most kHcDepth candidates nearest first, keep the
+//            longest common prefix up to min(kHcNice, matchlimit - p), the nearer one on a tie, stop at the cap.  Lengths
+//            (u8) and offsets (u16) go to the CTA's scratch in global memory (L2-resident); the lengths are then copied
+//            back into shared memory over the chains, which the parse no longer needs;
+//   parse  : warp 0 scans 32 positions per step: a position starts a match when its length is >= 4 and the next
+//            position's is not longer (lazy).  Lengths at the cap are extended with the same candidate.  Sequences are
+//            emitted 32 at a time (flush_seqs) into the scratch; the block is stored raw when that is not smaller;
+//   place  : the OFF chain gives the block's frame offset (as in sky_fused_kernel), and all warps copy it there.
+// This file is included by skychunk.cu after the fused kernel: it uses Params, BlockDesc, claim_block and the chain-word
+// accessors defined there.
+#pragma once
+
+namespace sky {
+
+#ifndef SKY_HC_DEPTH
+#define SKY_HC_DEPTH 16
+#endif
+constexpr uint32_t kHcDepth = SKY_HC_DEPTH;  // chain candidates walked per position
+constexpr uint32_t kHcHashBits = 14;         // head table: 1 << 14 entries
+constexpr uint32_t kHcNice = 32;             // a position's search stops at this length; the parse extends such matches
+constexpr int kHcWarps = 32;
+constexpr int kHcThreads = kHcWarps * 32;
+static_assert(kHcNice < 256 && kHcNice % 4 == 0, "lengths are kept as u8; the search compares 4 bytes at a time");
+
+struct HcCtl {
+    uint64_t in_full;   // the block's bulk copy has landed
+    BlockDesc desc;
+    uint32_t csize, raw, data_lo, data_hi;
+};
+constexpr uint32_t kHcInOff = 0;                                  // the block (+ slack for unaligned 4-byte reads)
+constexpr uint32_t kHcChainOff = kInBytes;                        // u16 per position; after the search: u8 length per position
+constexpr uint32_t kHcHeadOff = kHcChainOff + 2 * kBlock;         // u16 per hash
+constexpr uint32_t kHcCtlOff = kHcHeadOff + (2u << kHcHashBits);
+constexpr uint32_t kHcSmemBytes = kHcCtlOff + (uint32_t)sizeof(HcCtl);
+static_assert(kHcSmemBytes <= 232448, "one HC CTA per SM: at most 227 KiB of shared memory");
+// per-CTA scratch in global memory: lengths (u8), offsets (u16) and the compressed block
+constexpr uint32_t kHcLenOff = 0, kHcOffOff = kBlock, kHcOutOff = 3 * kBlock;
+constexpr uint32_t kHcScratchBytes = 4 * kBlock + 2048;
+
+__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    uint8_t *in = smem + kHcInOff;
+    HcCtl *ctl = reinterpret_cast<HcCtl *>(smem + kHcCtlOff);
+    const uint32_t in_s = smem_u32(in), chain_s = smem_u32(smem + kHcChainOff), head_s = smem_u32(smem + kHcHeadOff);
+    uint8_t *scr = p.scratch + (size_t)blockIdx.x * kHcScratchBytes;
+    uint8_t *g_len = scr + kHcLenOff;
+    uint16_t *g_off = reinterpret_cast<uint16_t *>(scr + kHcOffOff);
+    uint8_t *cout = scr + kHcOutOff;
+    if (tid == 0) {
+        mbar_init(&ctl->in_full, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    for (uint32_t in_phase = 0;; in_phase ^= 1) {
+        if (tid == 0) claim_block(p, &ctl->desc);
+        __syncthreads();  // (also: every warp is done with the previous block)
+        const BlockDesc d = ctl->desc;
+        if (!d.valid) break;
+        const uint32_t L = d.L;
+        if (tid == 0) {
+            const uint32_t bytes = (L + 15u) & ~15u;
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads of the old block before the async write
+            mbar_arrive_expect_tx(&ctl->in_full, bytes);
+            for (uint32_t o = 0; o < bytes; o += kLoadPiece) bulk_load(in + o, d.src + o, min(kLoadPiece, bytes - o), &ctl->in_full);
+        }
+        uint4 *h4 = reinterpret_cast<uint4 *>(smem + kHcHeadOff);
+        for (uint32_t k = tid; k < (2u << kHcHashBits) / 16; k += kHcThreads) h4[k] = make_uint4(0, 0, 0, 0);
+        mbar_wait(&ctl->in_full, in_phase);
+        __syncthreads();  // the head table is clear
+
+        const uint32_t mflimit = L - kMfLimit, matchlimit = L - kLastLiterals;  // (meaningful when L > kMfLimit)
+        const bool has_matches = L >= kMfLimit + 1;
+        // ---------------------------------------------------------------- chains (warp 0)
+        if (has_matches && warp == 0) {
+            for (uint32_t base = 0; base <= mflimit; base += 32) {
+                const uint32_t q = base + lane;
+                const bool valid = q <= mflimit;
+                const uint32_t h = valid ? (load32s(in_s, q) * 2654435761u) >> (32 - kHcHashBits) : 0x80000000u | lane;
+                const unsigned same = __match_any_sync(kFull, h);
+                const unsigned lower = same & ((1u << lane) - 1u);
+                const uint32_t prev = lower ? base + bfind(lower) + 1u : (valid ? lds16(head_s + h * 2u) : 0u);  // position + 1
+                __syncwarp();  // every read of head before any update
+                if (valid) {
+                    if ((same >> lane) == 1u) sts16(head_s + h * 2u, q + 1u);  // the highest lane of this hash
+                    sts16(chain_s + q * 2u, prev ? q + 1u - prev : 0u);
+                }
+                __syncwarp();
+            }
+        }
+        __syncthreads();
+        // ---------------------------------------------------------------- best match per position (all warps)
+        if (has_matches) {
+            for (uint32_t q = tid; q <= mflimit; q += kHcThreads) {
+                const uint32_t cap = min(kHcNice, matchlimit - q);
+                uint32_t best = 0, boff = 0, c = q, dist = lds16(chain_s + q * 2u);
+                for (uint32_t k = 0; k < kHcDepth && dist; k++) {
+                    c -= dist;
+                    // a longer match than `best` must agree at byte `best` (best < cap here): others are skipped unmeasured
+                    if (lds8(in_s + c + best) == lds8(in_s + q + best)) {
+                        uint32_t len = 0;
+                        for (;;) {
+                            const uint32_t x = load32s(in_s, q + len) ^ load32s(in_s, c + len);
+                            if (x) {
+                                len += (uint32_t)(__ffs(x) - 1) >> 3;
+                                break;
+                            }
+                            len += 4;
+                            if (len >= cap) break;
+                        }
+                        len = min(len, cap);
+                        if (len > best) {
+                            best = len;
+                            boff = q - c;
+                            if (best == cap) break;
+                        }
+                    }
+                    dist = lds16(chain_s + c * 2u);
+                }
+                g_len[q] = (uint8_t)(best >= kMinMatch ? best : 0u);
+                g_off[q] = (uint16_t)boff;
+            }
+        }
+        __syncthreads();
+        if (has_matches) {  // lengths back into shared memory, over the chains
+            const uint4 *src4 = reinterpret_cast<const uint4 *>(g_len);
+            uint4 *dst4 = reinterpret_cast<uint4 *>(smem + kHcChainOff);
+            for (uint32_t k = tid; k < (mflimit + 16u) / 16u; k += kHcThreads) dst4[k] = __ldcg(src4 + k);
+        }
+        __syncthreads();
+        // ---------------------------------------------------------------- lazy parse + emission (warp 0), then placement
+        if (warp == 0) {
+            uint32_t op = 0, anchor = 0;
+            if (has_matches) {
+                uint32_t cur = 0, nseq = 0, q0 = 0, q1 = 0;
+                for (;;) {
+                    if (cur <= mflimit) {
+                        const uint32_t x = cur + lane;
+                        const uint32_t len = x <= mflimit ? lds8(chain_s + x) : 0u;
+                        uint32_t nxt = __shfl_down_sync(kFull, len, 1);
+                        if (lane == 31) nxt = x + 1u <= mflimit ? lds8(chain_s + x + 1u) : 0u;
+                        const unsigned take = __ballot_sync(kFull, len >= kMinMatch && nxt <= len);
+                        if (!take) {
+                            cur += 32;
+                            continue;
+                        }
+                        const uint32_t f = (uint32_t)__ffs(take) - 1u, pos = cur + f;
+                        uint32_t ml = __shfl_sync(kFull, len, f);
+                        if (ml == kHcNice) ml = extend_coop_s(in_s, pos, pos - __ldcg(g_off + pos), ml, matchlimit - pos, lane);
+                        if (lane == nseq) {
+                            q0 = (pos - anchor) | (ml << 16);
+                            q1 = anchor | (pos << 16);  // (the offset is fetched for 32 sequences at once when they are emitted)
+                        }
+                        anchor = cur = pos + ml;
+                        if (++nseq < 32) continue;
+                    }
+                    if (nseq) {  // 32 sequences, or the last ones of the block
+                        if (lane < nseq) q1 = (q1 & 0xffffu) | ((uint32_t)__ldcg(g_off + (q1 >> 16)) << 16);
+                        op = flush_seqs(cout, op, in, q0, q1, nseq, false, lane);
+                        nseq = 0;
+                    }
+                    if (cur > mflimit) break;
+                }
+            }
+            op = emit_seq(cout, op, in, anchor, L - anchor, 0, 0, lane);  // the final literals
+            const bool raw = op > L - 1;  // LZ4F_makeBlock: a block that does not shrink is stored
+            if (lane == 0) {  // OFF chain: learn where this block starts, tell the successor at once
+                uint64_t *cw = p.chain + d.c;
+                uint64_t st;
+                unsigned ns = 128;
+                while (((st = ld_acquire(cw)) >> kOffBits) != d.j) {
+                    __nanosleep(ns);
+                    if (ns < 2048) ns <<= 1;
+                }
+                const uint64_t off = st & kOffMask;
+                const uint32_t bsize = raw ? L : op;
+                const uint64_t end = off + 4 + bsize;
+                if (!d.last) st_release(cw, ((uint64_t)(d.j + 1) << kOffBits) | end);
+                uint8_t *hdr = d.dst + off;
+                const uint32_t hword = raw ? (L | 0x80000000u) : op;
+                hdr[0] = (uint8_t)hword; hdr[1] = (uint8_t)(hword >> 8); hdr[2] = (uint8_t)(hword >> 16); hdr[3] = (uint8_t)(hword >> 24);
+                if (d.last) {
+                    uint8_t *e = d.dst + end;
+                    e[0] = e[1] = e[2] = e[3] = 0;  // EndMark
+                    p.out_len[d.c] = end + 4;
+                }
+                ctl->csize = bsize;
+                ctl->raw = raw;
+                ctl->data_hi = (uint32_t)((off + 4) >> 32);
+                ctl->data_lo = (uint32_t)(off + 4);
+            }
+        }
+        __syncthreads();
+        {   // the block to its final place: 16-byte-aligned slices per warp, straight from the input when stored raw
+            uint8_t *out = d.dst + (((uint64_t)ctl->data_hi << 32) | ctl->data_lo);
+            const uint32_t n = ctl->csize;
+            const uint32_t per = (((n + kHcWarps - 1) / kHcWarps) + 15u) & ~15u;
+            const uint32_t lo = warp * per;
+            if (lo < n) {
+                if (ctl->raw) warp_copy_stream<true>(out + lo, d.src + lo, min(per, n - lo), lane);
+                else warp_copy_stream<false>(out + lo, cout + lo, min(per, n - lo), lane);
+            }
+        }
+    }
+}
+
+}  // namespace sky

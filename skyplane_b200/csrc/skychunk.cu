@@ -623,6 +623,8 @@ __global__ void sky_box_setup_kernel(BoxChunk *bc, uint64_t *blk_base, const Chu
 
 }  // namespace sky
 
+#include "lz4hc.cuh"
+
 // ======================================================================================= host side
 using namespace sky;
 
@@ -669,6 +671,11 @@ struct BatchMeta {  // one batch's descriptors and results (the receiver uses th
     DevMem<uint32_t> counters;
     DevMem<uint8_t> scratch;  // compress scratch: kScratchBytes per CTA of the grid (kernels of different slots overlap)
 };
+struct HcArrays {  // SKY_F_HC: the HC kernel's scratch, and the stream the digests run on beside it (fork / join events)
+    DevMem<uint8_t> scratch;  // kHcScratchBytes per CTA (one CTA per SM)
+    Stream md5_stream;
+    Event ev_fork, ev_join;
+};
 struct DecodeArrays {  // receiver side
     PinnedMem<DecChunk> h_chunks; DevMem<DecChunk> d_chunks;
     PinnedMem<int32_t> h_status; DevMem<int32_t> d_status;
@@ -702,6 +709,7 @@ struct Slot {
     BatchMeta meta;
     DecodeArrays dec;
     BoxArrays box;
+    HcArrays hc;
     Ticket ticket;
 };
 
@@ -725,6 +733,8 @@ struct sky_ctx {
         if (st_d2h) cudaStreamSynchronize(st_d2h);
         for (Slot &s : slots)
             if (s.stream) cudaStreamSynchronize(s.stream);
+        for (Slot &s : slots)
+            if (s.hc.md5_stream) cudaStreamSynchronize(s.hc.md5_stream);
     }
 };
 
@@ -779,6 +789,17 @@ static int alloc_dec(sky_ctx *ctx, DecodeArrays &d) {
     CK(ctx, cudaMalloc(a.d_status.put(), nc * sizeof(int32_t)));
     CK(ctx, cudaMalloc(a.d_dec_done.put(), nc * sizeof(uint32_t)));
     d = std::move(a);
+    return SKY_OK;
+}
+
+static int alloc_hc(sky_ctx *ctx, HcArrays &h) {
+    if (h.scratch) return SKY_OK;
+    HcArrays a;
+    CK(ctx, cudaMalloc(a.scratch.put(), (size_t)ctx->sm_count * kHcScratchBytes));
+    CK(ctx, cudaStreamCreateWithFlags(a.md5_stream.put(), cudaStreamNonBlocking));
+    CK(ctx, cudaEventCreateWithFlags(a.ev_fork.put(), cudaEventDisableTiming));
+    CK(ctx, cudaEventCreateWithFlags(a.ev_join.put(), cudaEventDisableTiming));
+    h = std::move(a);
     return SKY_OK;
 }
 
@@ -864,6 +885,9 @@ uint32_t sky_kernel_config(int what) {
     case 1: return (uint32_t)kWarps;
     case 2: return kSegSlots;
     case 3: return kMaxStepLog;
+    case 4: return kHcDepth;
+    case 5: return kHcHashBits;
+    case 6: return kHcNice;
     default: return 0;
     }
 }
@@ -892,6 +916,7 @@ int sky_ctx_create(int device, uint64_t max_batch_bytes, uint32_t max_chunks, ui
     CK(ctx, cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
     cudaError_t e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_hc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
     if (e != cudaSuccess) {
         g_err = ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (this build carries sm_90a code only)";
         return SKY_E_CUDA;
@@ -1006,12 +1031,19 @@ static uint32_t fill_md5_order(uint32_t *order, uint32_t n, const uint64_t *len)
     return ng;
 }
 
+// SKY_F_HC selects how frames are made, so it needs SKY_F_LZ4, or no stage bit at all (= LZ4 + MD5).
+static bool hc_flags_valid(uint32_t flags) { return !(flags & SKY_F_HC) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5; }
+
 // Fills the slot's metadata for a batch and enqueues: meta H2D, counter reset, fused kernel, results D2H.
 // `meta_st`: stream the three small metadata copies ride on (the H2D stream on the host path, so they are
 // never queued behind another batch's frame copies); `st`: the stream the kernel runs on.
 static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t meta_st, uint32_t n, const uint8_t *d_src,
                         const uint64_t *src_off, const uint64_t *src_len, uint8_t *d_dst, const uint64_t *dst_off, uint32_t flags) {
     if ((flags & (SKY_F_LZ4 | SKY_F_MD5)) == 0) flags |= SKY_F_LZ4 | SKY_F_MD5;
+    if (flags & SKY_F_HC) {
+        const int hrc = alloc_hc(ctx, s.hc);
+        if (hrc != SKY_OK) return hrc;
+    }
     BatchMeta &m = s.meta;
     uint32_t rows;
     int rc = batch_geometry(n, src_len, rows, [&](uint32_t i, uint32_t nblk) {
@@ -1051,8 +1083,29 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
     p.rows = rows;
     p.flags = flags;
     CK(ctx, cudaEventRecord(s.ev_k0, st));
-    sky_fused_kernel<<<grid, kThreads, kSmemBytes, st>>>(p);
-    CK(ctx, cudaGetLastError());
+    if (flags & SKY_F_HC) {
+        // high-ratio frames from sky_hc_kernel; the digests from the fused kernel's MD5-only mode on a forked stream, so
+        // the two run side by side (the HC kernel's CTAs take the SMs as the digest CTAs leave them)
+        HcArrays &h = s.hc;
+        const bool md5 = (flags & SKY_F_MD5) != 0;
+        if (md5) {
+            CK(ctx, cudaEventRecord(h.ev_fork, st));
+            CK(ctx, cudaStreamWaitEvent(h.md5_stream, h.ev_fork, 0));
+            Params pm = p;
+            pm.flags = SKY_F_MD5;
+            sky_fused_kernel<<<grid, kThreads, kSmemBytes, h.md5_stream>>>(pm);
+            CK(ctx, cudaGetLastError());
+            CK(ctx, cudaEventRecord(h.ev_join, h.md5_stream));
+            ctx->launches++;
+        }
+        p.scratch = h.scratch;
+        sky_hc_kernel<<<ctx->sm_count, kHcThreads, kHcSmemBytes, st>>>(p);
+        CK(ctx, cudaGetLastError());
+        if (md5) CK(ctx, cudaStreamWaitEvent(st, h.ev_join, 0));
+    } else {
+        sky_fused_kernel<<<grid, kThreads, kSmemBytes, st>>>(p);
+        CK(ctx, cudaGetLastError());
+    }
     CK(ctx, cudaEventRecord(s.ev_k1, st));
     ctx->launches++;
     if (flags & SKY_F_E2EE) {
@@ -1095,6 +1148,7 @@ int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64
                        uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
     if (!ctx || n == 0 || !src_off || !src_len || !dst_off || !dst_cap || !d_dst) return SKY_E_INVALID;
     if (flags & SKY_F_E2EE) return SKY_E_INVALID;  // boxes are a host-path feature (sky_submit)
+    if (!hc_flags_valid(flags)) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
     if ((reinterpret_cast<uintptr_t>(d_src) & 15) || (reinterpret_cast<uintptr_t>(d_dst) & 15)) return SKY_E_INVALID;
     for (uint32_t i = 0; i < n; i++) {
@@ -1117,7 +1171,7 @@ int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64
 
 int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t *src_len, void *const *dst,
                const uint64_t *dst_cap, uint32_t flags, const uint8_t *nonces, uint64_t *ticket) {
-    if (!ctx || n == 0 || !src || !src_len || !ticket) return SKY_E_INVALID;
+    if (!ctx || n == 0 || !src || !src_len || !ticket || !hc_flags_valid(flags)) return SKY_E_INVALID;
     if ((flags & (SKY_F_LZ4 | SKY_F_MD5)) == 0) flags |= SKY_F_LZ4 | SKY_F_MD5;
     const bool e2ee = (flags & SKY_F_E2EE) != 0, frames = (flags & SKY_F_LZ4) != 0;
     const bool returns_data = frames || e2ee;  // MD5-only without E2EE: only digests come back

@@ -55,10 +55,12 @@ def run_stream(
     warmup_requests: int = 0,
     operator_cls=GatewayCompressHash,
     n_slots: int = 4,
+    high_ratio: bool = False,
 ) -> Dict:
     """Stream ``n_requests`` chunk requests (recycling ``pool_files`` by hard link) through the operator.
 
     The first ``warmup_requests`` completions are not timed (worker start-up: CUDA context, pinned staging).
+    ``high_ratio`` is handed to the operator (GatewayCompressHash's high-ratio frames) when set.
     Returns {"wall_s", "bytes", "records": [{chunk_id, pool_index, md5, raw_len, frame_path}], "status": {...}}.
     """
     chunk_dir = Path(chunk_dir)
@@ -69,6 +71,7 @@ def run_stream(
     op = operator_cls(
         "compress_hash", "local:box", qin, qout, err_ev, err_q, store, n_processes=n_workers,
         max_batch_chunks=max_batch_chunks, max_batch_bytes=max_batch_bytes, n_gpus=n_gpus, keep_frames_on_disk=keep_frames, n_slots=n_slots,
+        **({"high_ratio": True} if high_ratio else {}),
     )
     op.start_workers()
     records: List[Dict] = []

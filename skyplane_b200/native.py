@@ -14,7 +14,7 @@ LIB_PATH = _PKG / "libskychunk.so"
 
 SKY_OK = 0
 SKY_E_INVALID, SKY_E_NOGPU, SKY_E_CUDA, SKY_E_CAPACITY, SKY_E_BUSY, SKY_E_TICKET, SKY_E_NOMEM, SKY_E_NOKEY = -1, -2, -3, -4, -5, -6, -7, -8
-F_LZ4, F_MD5, F_E2EE = 1, 2, 16
+F_LZ4, F_MD5, F_E2EE, F_HC = 1, 2, 16, 32
 BOX_OVERHEAD = 40
 # sky_decode status codes
 D_OK, D_BAD_HEADER, D_CORRUPT, D_SIZE, D_UNSUPPORTED, D_LAYOUT, D_TRUNCATED, D_AUTH = 0, -1, -2, -3, -4, -5, -6, -7
@@ -128,10 +128,11 @@ def device_pci_bus_id(device: int) -> str:
 
 
 def kernel_config() -> dict:
-    """Compile-time constants of the loaded build (sky_kernel_config)."""
+    """Compile-time constants of the loaded build (sky_kernel_config); the hc_* keys read 0 on a library without F_HC."""
     L = lib()
     return {"lz4_entries": L.sky_kernel_config(0), "warps": L.sky_kernel_config(1), "seg_slots": L.sky_kernel_config(2),
-            "max_step_log": L.sky_kernel_config(3)}
+            "max_step_log": L.sky_kernel_config(3), "hc_depth": L.sky_kernel_config(4), "hc_hash_bits": L.sky_kernel_config(5),
+            "hc_nice": L.sky_kernel_config(6)}
 
 
 def frame_bound(n: int) -> int:

@@ -133,15 +133,21 @@ class GatewayCompressHash(GatewayOperator):
         e2ee_key_bytes: Optional[bytes] = None,
         sink=None,
         n_slots: int = 4,
+        high_ratio: bool = False,
     ):
         """use_compression / e2ee_key_bytes: GatewaySender's arguments of the same name (gateway_operator.py:154-168):
         ``use_compression=False`` digests the chunk and lets it pass through uncompressed (``is_compressed=False``);
         ``e2ee_key_bytes`` seals every payload in a SecretBox on the GPU.
+        high_ratio: frames from the high-ratio parse (``ChunkStage.launch(hc=True)``): same frame format and receiver,
+        fewer bytes on the wire for more GPU time per chunk.  Needs ``use_compression``.
         sink: ``callable(worker_id) -> socket``, called once in each worker.  With a sink the worker sends every payload
         straight from the pinned staging slot (``wire.send_results``: WireProtocolHeader + payload, no intermediate bytes
         object, no frame file) -- the tail of ``GatewaySender.process`` (gateway_operator.py:367-402)."""
         super().__init__(handle, region, input_queue, output_queue, error_event, error_queue, chunk_store, n_processes)
         self.use_compression = True if use_compression is None else bool(use_compression)
+        if high_ratio and not self.use_compression:
+            raise ValueError("high_ratio selects how chunks are compressed: it needs use_compression")
+        self.high_ratio = bool(high_ratio)
         self.e2ee_key_bytes = e2ee_key_bytes
         self.sink = sink
         # batches in flight per worker: a batch of 8 MiB chunks spends >= 70 ms on the GPU whatever its size (one serial MD5
@@ -284,7 +290,10 @@ class GatewayCompressHash(GatewayOperator):
         if not all([fut.result() for _, fut in jobs]):
             stage.release(slot)
             return False
-        stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None)
+        if self.high_ratio:
+            stage.launch(slot, compress=True, encrypt=self.e2ee_key_bytes is not None, hc=True)
+        else:
+            stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None)
         return True
 
     def _launch(self, reqs: List[ChunkRequest]):

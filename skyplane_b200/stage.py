@@ -150,14 +150,19 @@ class ChunkStage:
         self.ctx.set_e2ee_key(key)
         self._has_key = key is not None
 
-    def launch(self, slot: _Slot, compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None) -> _Slot:
+    def launch(self, slot: _Slot, compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None, hc: bool = False) -> _Slot:
         """compress=False is the reference's `compress: false` (digest only, the chunk passes through);
-        encrypt=True seals every payload with the stage's key (nonces: 24 bytes per chunk, default os.urandom)."""
+        encrypt=True seals every payload with the stage's key (nonces: 24 bytes per chunk, default os.urandom);
+        hc=True makes the frames with the high-ratio parse (F_HC): same frame format, fewer bytes, more GPU time."""
         if not slot.lens:
             raise ValueError("empty batch")
+        if hc and not compress:
+            raise ValueError("hc=True selects how frames are compressed: it needs compress=True")
+        if hc and not native.kernel_config()["hc_depth"]:
+            raise native.SkyChunkError(native.SKY_E_INVALID, f"{native.LIB_PATH.name} was built without the high-ratio kernel (F_HC)")
         base_in, base_out = slot.inp.addr, slot.out.addr
         src = [base_in + o for o in slot.in_off]
-        flags = native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0)
+        flags = native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0) | (native.F_HC if hc else 0)
         if encrypt and nonces is None:
             nonces = os.urandom(24 * len(slot.lens))  # what nacl.utils.random(24) draws per message
         if compress or encrypt:
@@ -181,8 +186,9 @@ class ChunkStage:
         return res
 
     # ------------------------------------------------------------------ sync convenience
-    def process(self, chunks: Sequence[BytesLike], compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None) -> List[StageResult]:
-        """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes."""
+    def process(self, chunks: Sequence[BytesLike], compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None,
+                hc: bool = False) -> List[StageResult]:
+        """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes (hc: see launch)."""
         out: List[StageResult] = []
         i = 0
         while i < len(chunks):
@@ -194,7 +200,7 @@ class ChunkStage:
             if j == i:
                 self.release(slot)
                 raise native.SkyChunkError(native.SKY_E_CAPACITY, f"chunk of {memoryview(chunks[i]).nbytes} bytes exceeds max_batch_bytes")
-            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None)
+            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc)
             for r in self.collect(slot):
                 out.append(StageResult(frame=memoryview(bytes(r.frame)), md5=r.md5, raw_len=r.raw_len, comp_len=r.comp_len,
                                        is_compressed=r.is_compressed, is_encrypted=r.is_encrypted))

@@ -1,10 +1,16 @@
 #!/usr/bin/env python
 """Kernel-only sweeps on one GPU (device-resident inputs): stage flags x workload x chunk size.
-Writes one JSON line per configuration.  Used to fill profiles/ and DESIGN.md tables; not a bench line."""
+Writes one JSON line per configuration.  Used to fill profiles/ and DESIGN.md tables; not a bench line.
+Flag sets: lz4, md5, both (the fused kernel), hc (SKY_F_HC: high-ratio frames + MD5), hc-lz4 (high-ratio frames only).
+--ref-ratio adds the reference's ratio (liblz4 level 0, linked blocks) on the distinct chunks; --liblz4-level9 times liblz4
+level 9 with independent blocks on all of the host's cores (the rate the reference's sender would get from that level)."""
 import argparse
 import json
+import multiprocessing as mp
+import os
 import statistics
 import sys
+import time
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
@@ -36,6 +42,32 @@ def make_input(workload, n_chunks, chunk_bytes, dev):
     return buf, stride
 
 
+def pool_chunks(workload, chunk_bytes):
+    """The distinct chunks make_input cycles through (Silesia-like workloads), as host bytes."""
+    base = min(chunk_bytes, 16 << 20)
+    return [(synth.silesia_like_chunk(2000 + i, base) * (chunk_bytes // base + 1))[:chunk_bytes] for i in range(8)]
+
+
+def _level9_size(data):
+    from tools import hc_model
+
+    return len(hc_model.liblz4_frame(data, 9))
+
+
+def liblz4_level9_all_cores(chunks, rounds=2):
+    """liblz4 level 9, independent 64 KiB blocks, one chunk per process on every core: -> (GB/s of raw input, ratio)."""
+    n = os.cpu_count() or 1
+    work = [c for _ in range(rounds) for c in chunks]
+    work = (work * (n // len(work) + 1))[: max(n, len(work))]
+    with mp.get_context("fork").Pool(n) as pool:
+        pool.map(_level9_size, work[:n])  # warm the workers (library load)
+        t = time.perf_counter()
+        sizes = pool.map(_level9_size, work, chunksize=1)
+        dt = time.perf_counter() - t
+    raw = sum(map(len, work))
+    return {"liblz4_level9_indep_cores": n, "liblz4_level9_gbs": raw / dt / 1e9, "liblz4_level9_ratio": raw / sum(sizes)}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--total-mib", type=int, default=2048)
@@ -44,13 +76,27 @@ def main():
     ap.add_argument("--flags", default="lz4,md5,both")
     ap.add_argument("--iters", type=int, default=3)
     ap.add_argument("--decode", action="store_true", help="also time the receiver-side decode + MD5 of the frames")
+    ap.add_argument("--decode-from", default="both", help="flag set whose frames --decode times (both, hc)")
+    ap.add_argument("--ref-ratio", action="store_true", help="also the reference's ratio on the distinct chunks (CPU)")
+    ap.add_argument("--liblz4-level9", action="store_true", help="also liblz4 level 9 on all host cores (CPU)")
     a = ap.parse_args()
     dev = torch.device("cuda", 0)
-    FL = {"lz4": native.F_LZ4, "md5": native.F_MD5, "both": 0}
+    FL = {"lz4": native.F_LZ4, "md5": native.F_MD5, "both": 0, "hc": native.F_HC, "hc-lz4": native.F_HC | native.F_LZ4}
     for wl in a.workloads.split(","):
         for sz in a.sizes_mib.split(","):
             chunk_bytes = int(float(sz) * (1 << 20))
             n = max(1, (a.total_mib << 20) // chunk_bytes)
+            # (CPU legs first: their worker processes fork before this process has a CUDA context)
+            if wl == "silesia" and (a.ref_ratio or a.liblz4_level9):
+                import oracle.reflib as ref
+
+                chunks = pool_chunks(wl, chunk_bytes)
+                row = {"workload": wl, "chunk_mib": float(sz), "distinct_chunks": len(chunks)}
+                if a.ref_ratio:
+                    row["reference_ratio"] = sum(map(len, chunks)) / sum(len(ref.lz4f_compress(c)) for c in chunks)
+                if a.liblz4_level9:
+                    row.update(liblz4_level9_all_cores(chunks))
+                print(json.dumps(row), flush=True)
             d_in, stride = make_input(wl, n, chunk_bytes, dev)
             bound = native.frame_bound(chunk_bytes)
             so = native.round16(bound)
@@ -71,7 +117,8 @@ def main():
                                   "ratio": (tot / sum(out_lens)) if sum(out_lens) else None, "per_stream_gbs": chunk_bytes / k / 1e6}), flush=True)
             if a.decode:
                 # receiver side: decode the frames just produced (d_out) back into a fresh buffer + MD5 of the result
-                out_lens, dg, _ = ctx.process_device(d_in.data_ptr(), src_off, [chunk_bytes] * n, d_out.data_ptr(), dst_off, [bound] * n, 0, 0)
+                out_lens, dg, _ = ctx.process_device(d_in.data_ptr(), src_off, [chunk_bytes] * n, d_out.data_ptr(), dst_off, [bound] * n,
+                                                     FL[a.decode_from], 0)
                 d_back = torch.empty_like(d_in)
                 ms = []
                 for it in range(a.iters + 1):
@@ -80,7 +127,7 @@ def main():
                         ms.append(kms)
                 ok = all(x == 0 for x in st) and dg2 == dg and bool(torch.equal(d_back[: n * stride - (stride - chunk_bytes)], d_in[: n * stride - (stride - chunk_bytes)]))
                 k = statistics.median(ms)
-                print(json.dumps({"workload": wl, "chunk_mib": float(sz), "chunks": n, "flags": "decode+md5", "kernel_ms": k,
+                print(json.dumps({"workload": wl, "chunk_mib": float(sz), "chunks": n, "flags": "decode+md5", "frames_from": a.decode_from, "kernel_ms": k,
                                   "raw_output_gbs": n * chunk_bytes / k / 1e6, "roundtrip_ok": ok}), flush=True)
                 del d_back
             ctx.close()

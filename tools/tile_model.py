@@ -68,13 +68,17 @@ def blocks(data: bytes, o: Opts):
     return out
 
 
-def frame(data: bytes, o: Opts | None = None) -> bytes:
-    o = o or kernel_opts()
-    if not data:
+def assemble(n: int, blks) -> bytes:
+    """The stage's frame around an n-byte chunk's blocks [(compressed size or 0 when stored raw, block bytes)]."""
+    if not n:
         d = bytes([0x60, 0x40])
         return bytes([0x04, 0x22, 0x4D, 0x18]) + d + bytes([(_xxh32_small(d) >> 8) & 0xFF]) + bytes(4)
-    d = bytes([0x68, 0x40]) + len(data).to_bytes(8, "little")
+    d = bytes([0x68, 0x40]) + n.to_bytes(8, "little")
     fr = bytearray(bytes([0x04, 0x22, 0x4D, 0x18]) + d + bytes([(_xxh32_small(d) >> 8) & 0xFF]))
-    for c, b in blocks(data, o):
+    for c, b in blks:
         fr += (c if c else (len(b) | 0x80000000)).to_bytes(4, "little") + b
     return bytes(fr + bytes(4))
+
+
+def frame(data: bytes, o: Opts | None = None) -> bytes:
+    return assemble(len(data), blocks(data, o or kernel_opts()))
