@@ -146,7 +146,9 @@ __device__ __forceinline__ uint32_t xxh32_small(const uint8_t *p, uint32_t len) 
     return h;
 }
 
-// Writes the frame header for an n-byte chunk at dst; returns its size (15, or 7 when n == 0).
+constexpr uint32_t kFrameHeaderBytes = 15;  // frame header with content size: magic, FLG, BD, 8-byte content size, header checksum
+
+// Writes the frame header for an n-byte chunk at dst; returns its size (kFrameHeaderBytes, or 7 when n == 0).
 // Single thread.
 __device__ __forceinline__ uint32_t write_frame_header(uint8_t *dst, uint64_t n) {
     uint8_t d[10];
@@ -163,8 +165,8 @@ __device__ __forceinline__ uint32_t write_frame_header(uint8_t *dst, uint64_t n)
     for (int i = 0; i < 8; i++) d[2 + i] = (uint8_t)(n >> (8 * i));
 #pragma unroll
     for (int i = 0; i < 10; i++) dst[4 + i] = d[i];
-    dst[14] = (uint8_t)(xxh32_small(d, 10) >> 8);
-    return 15;
+    dst[kFrameHeaderBytes - 1] = (uint8_t)(xxh32_small(d, 10) >> 8);
+    return kFrameHeaderBytes;
 }
 
 // ---- sequence emission ----------------------------------------------------------------------------

@@ -15,10 +15,10 @@
 //   parse  : warp 0 scans 32 positions per step: a position starts a match when its length is >= 4 and the next
 //            position's is not longer (lazy).  Lengths at the cap are extended with the same candidate.  Sequences are
 //            emitted 32 at a time (flush_seqs) into the scratch; the block is stored raw when that is not smaller;
-//   place  : the OFF chain gives the block's frame offset (as in sky_fused_kernel), and all warps copy it there.
-// This file is included by skychunk.cu after the fused kernel: it uses Params, BlockDesc, claim_block and the chain-word
-// accessors defined there.
+//   place  : the OFF chain gives the block's frame offset (place_block), and all warps copy it there.
+// Claim, load, placement and write-out are frame.cuh's, shared with sky_fused_kernel.
 #pragma once
+#include "frame.cuh"
 
 namespace sky {
 
@@ -35,7 +35,8 @@ static_assert(kHcNice < 256 && kHcNice % 4 == 0, "lengths are kept as u8; the se
 struct HcCtl {
     uint64_t in_full;   // the block's bulk copy has landed
     BlockDesc desc;
-    uint32_t csize, raw, data_lo, data_hi;
+    uint64_t data;  // frame offset of the block's first data byte
+    uint32_t csize, raw;
 };
 constexpr uint32_t kHcInOff = 0;                                  // the block (+ slack for unaligned 4-byte reads)
 constexpr uint32_t kHcChainOff = kInBytes;                        // u16 per position; after the search: u8 length per position
@@ -69,12 +70,7 @@ __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
         const BlockDesc d = ctl->desc;
         if (!d.valid) break;
         const uint32_t L = d.L;
-        if (tid == 0) {
-            const uint32_t bytes = (L + 15u) & ~15u;
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads of the old block before the async write
-            mbar_arrive_expect_tx(&ctl->in_full, bytes);
-            for (uint32_t o = 0; o < bytes; o += kLoadPiece) bulk_load(in + o, d.src + o, min(kLoadPiece, bytes - o), &ctl->in_full);
-        }
+        if (tid == 0) load_block(in, d.src, L, &ctl->in_full);
         uint4 *h4 = reinterpret_cast<uint4 *>(smem + kHcHeadOff);
         for (uint32_t k = tid; k < (2u << kHcHashBits) / 16; k += kHcThreads) h4[k] = make_uint4(0, 0, 0, 0);
         mbar_wait(&ctl->in_full, in_phase);
@@ -174,44 +170,18 @@ __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
                 }
             }
             op = emit_seq(cout, op, in, anchor, L - anchor, 0, 0, lane);  // the final literals
-            const bool raw = op > L - 1;  // LZ4F_makeBlock: a block that does not shrink is stored
-            if (lane == 0) {  // OFF chain: learn where this block starts, tell the successor at once
-                uint64_t *cw = p.chain + d.c;
-                uint64_t st;
-                unsigned ns = 128;
-                while (((st = ld_acquire(cw)) >> kOffBits) != d.j) {
-                    __nanosleep(ns);
-                    if (ns < 2048) ns <<= 1;
-                }
-                const uint64_t off = st & kOffMask;
-                const uint32_t bsize = raw ? L : op;
-                const uint64_t end = off + 4 + bsize;
-                if (!d.last) st_release(cw, ((uint64_t)(d.j + 1) << kOffBits) | end);
-                uint8_t *hdr = d.dst + off;
-                const uint32_t hword = raw ? (L | 0x80000000u) : op;
-                hdr[0] = (uint8_t)hword; hdr[1] = (uint8_t)(hword >> 8); hdr[2] = (uint8_t)(hword >> 16); hdr[3] = (uint8_t)(hword >> 24);
-                if (d.last) {
-                    uint8_t *e = d.dst + end;
-                    e[0] = e[1] = e[2] = e[3] = 0;  // EndMark
-                    p.out_len[d.c] = end + 4;
-                }
-                ctl->csize = bsize;
-                ctl->raw = raw;
-                ctl->data_hi = (uint32_t)((off + 4) >> 32);
-                ctl->data_lo = (uint32_t)(off + 4);
+            if (lane == 0) {
+                const BlockPlace pl = place_block(p, d, op, L);
+                ctl->data = pl.data;
+                ctl->csize = op;
+                ctl->raw = pl.raw;
             }
         }
         __syncthreads();
-        {   // the block to its final place: 16-byte-aligned slices per warp, straight from the input when stored raw
-            uint8_t *out = d.dst + (((uint64_t)ctl->data_hi << 32) | ctl->data_lo);
-            const uint32_t n = ctl->csize;
-            const uint32_t per = (((n + kHcWarps - 1) / kHcWarps) + 15u) & ~15u;
-            const uint32_t lo = warp * per;
-            if (lo < n) {
-                if (ctl->raw) warp_copy_stream<true>(out + lo, d.src + lo, min(per, n - lo), lane);
-                else warp_copy_stream<false>(out + lo, cout + lo, min(per, n - lo), lane);
-            }
-        }
+        // the block to its final place, straight from the input when stored raw
+        uint8_t *out = d.dst + ctl->data;
+        if (ctl->raw) copy_block<kHcWarps, true>(out, d.src, L, warp, lane);
+        else copy_block<kHcWarps, false>(out, cout, ctl->csize, warp, lane);
     }
 }
 

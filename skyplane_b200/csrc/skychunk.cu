@@ -9,12 +9,11 @@
 //                   every chunk, then row j+1 ...): bulk-load the block into shared memory, warps 0-1 probe, warps 2-13
 //                   parse segment by segment into an L2-resident scratch (lz4.cuh), warp 0 plans the block's layout.
 // Output placement (single pass, no compaction kernel): a block's final place in the frame is only known when every block
-// before it has been sized, so one per-chunk word orders the blocks:
-//   OFF = (next block index << 40) | frame offset of that block: a prefix sum handed from block j-1 to block j as soon as
-//         j-1 knows its compressed size -- before it has written a byte, so offsets race down the chain.
-// Block j sizes itself from its segments' records, waits for OFF (its final position), publishes OFF for j+1 and then
-// writes its bytes to the final place exactly once (stored blocks straight from the input).  The last block's CTA writes
-// the EndMark and the frame length.
+// before it has been sized, so one per-chunk word, the OFF chain (frame.cuh), orders the blocks.  Block j sizes itself
+// from its segments' records, takes its frame offset from the chain and passes it on (place_block), then writes its bytes
+// to the final place exactly once (stored blocks straight from the input).  The last block's CTA writes the EndMark and
+// the frame length.  The high-ratio compressor (lz4hc.cuh, SKY_F_HC) claims, loads and places its blocks through the
+// same frame.cuh helpers.
 //
 // The two roles never wait on each other: digest lanes and compressors each read their own input from HBM.
 //
@@ -37,8 +36,10 @@
 #include <vector>
 
 #include "../../include/skychunk.h"
+#include "frame.cuh"
 #include "lz4.cuh"
 #include "lz4dec.cuh"
+#include "lz4hc.cuh"
 #include "md5.cuh"
 #include "secretbox.cuh"
 
@@ -57,19 +58,10 @@ constexpr int kThreads = kWarps * 32;
 constexpr int kRing = kParsers + SKY_RING_EXTRA;       // segment slots between the prober and the parsers
 constexpr int kMd5WarpsPerCta = 4;        // digest CTAs run 4 MD5 groups (one per SM sub-partition), see sky_fused_kernel
 constexpr uint32_t kRingBytes = SKY_MD5_SLOTS * 2048;  // MD5 staging ring: slots x 64 B x 32 lanes
-constexpr uint32_t kLoadPiece = 8192;     // bytes per bulk copy of the block load
 constexpr int kCtasPerSm = 2;             // fused kernel: 2 x ~110 KiB of shared memory per SM
 constexpr uint64_t kMaxChunkBlocks = 1ull << 21;  // 64 KiB blocks = 128 GiB per chunk: md5_warp counts 64-byte blocks in 32 bits
-constexpr int kOffBits = 40;
-constexpr uint64_t kOffMask = (1ull << kOffBits) - 1;
 
 // ---- shared-memory layout of the fused kernel (dynamic, 128-byte aligned base) -------------------------
-struct BlockDesc {            // written by the prober's lane 0, read by every warp after the block-start barrier
-    const uint8_t *src;       // block start in the chunk (16-byte aligned)
-    uint8_t *dst;             // chunk's frame region
-    uint32_t c, j, L, last;   // chunk, block index, block length, 1 = last block of the chunk
-    uint32_t valid, pad;
-};
 struct Ctl {
     uint64_t in_full;               // bulk copy of the block has landed
     uint64_t full[kRing], empty[kRing];
@@ -78,10 +70,9 @@ struct Ctl {
     volatile uint32_t block_end_seq;  // sequence number after the current block's last segment (0xffffffff while probing)
     volatile uint32_t nseg;
     volatile uint32_t seg_hit[4];     // per segment (mod 4): OR of its batches' hit masks (decides the stride two segments on)
-    uint32_t csize, raw, last_lits, tail_off;   // plan results: compressed size, stored?, final literal run and where it goes
-    uint32_t data_lo, data_hi;                  // frame offset of the block's first data byte
+    uint32_t raw, last_lits, tail_off;  // plan results: stored?, final literal run and where it goes
+    uint64_t data;                      // frame offset of the block's first data byte
 };
-constexpr uint32_t kInBytes = kBlock + 128;    // + slack: unaligned 4-byte reads may touch the word after the last byte
 constexpr uint32_t kInOff = 0;
 constexpr uint32_t kTabOff = kInOff + kInBytes;
 constexpr uint32_t kRingOff = kTabOff + kTableBytes;
@@ -94,96 +85,17 @@ static_assert(kEntries % 128 == 0, "SKY_LZ4_ENTRIES must be a multiple of 128");
 static_assert(kMd5WarpsPerCta * kRingBytes <= kInBytes, "the MD5 rings live in the block buffer of a digest CTA");
 static_assert(sizeof(SegSlot) % 16 == 0 && sizeof(SegRec) == 16 && sizeof(SegPlan) == 16, "layout");
 
-struct ChunkDesc {
-    const uint8_t *src;  // 16-byte aligned
-    uint8_t *dst;        // 16-byte aligned
-    uint64_t len;
-    uint32_t nblk;
-};
-
-struct Params {
-    const ChunkDesc *chunks;
-    const uint32_t *md5_order;  // chunk indices, longest first, padded with 0xffffffff to 32*n_groups
-    uint64_t *chain;            // per chunk OFF word: (next block index << 40) | frame offset of that block
-    uint64_t *out_len;          // per chunk frame length
-    uint8_t *md5_out;           // 16 bytes per chunk
-    uint32_t *counters;         // [0] = LZ4 work counter
-    uint8_t *scratch;           // kScratchBytes per CTA: where a block's segments are compressed before its frame offset is known
-    uint32_t n_chunks;
-    uint32_t n_groups;
-    uint32_t n_md5_ctas;        // CTAs 0..n_md5_ctas-1 digest (4 groups each at a time) before they compress
-    uint32_t rows;  // max(1, max nblk)
-    uint32_t flags;
-};
-
-__device__ __forceinline__ uint64_t ld_acquire(const uint64_t *p) {
-    uint64_t v;
-    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ uint32_t ld_acquire32(const uint32_t *p) {
-    uint32_t v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ uint32_t ld_relaxed32(const uint32_t *p) {
-    uint32_t v;
-    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release(uint64_t *p, uint64_t v) {
-    asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ void st_release32(uint32_t *p, uint32_t v) {
-    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
 // named-barrier token between the two prober warps: the releaser arrives, the waiter syncs (ids 1 and 2, 64 threads)
 template <int kId>
 __device__ __forceinline__ void bar_arrive() { asm volatile("bar.arrive %0, 64;" ::"n"(kId) : "memory"); }
 template <int kId>
 __device__ __forceinline__ void bar_wait() { asm volatile("bar.sync %0, 64;" ::"n"(kId) : "memory"); }
 
-// Prober lane 0: claim the next block that has LZ4 work (empty chunks are finished on the spot) and describe it to the CTA.
-__device__ __forceinline__ void claim_block(const Params &p, BlockDesc *d) {
-    const uint32_t total = p.rows * p.n_chunks;
-    for (;;) {
-        const uint32_t w = atomicAdd(p.counters, 1u);
-        if (w >= total) {
-            d->valid = 0;
-            return;
-        }
-        const uint32_t c = w % p.n_chunks, j = w / p.n_chunks;  // row-major: block row j of every chunk, then row j+1
-        const ChunkDesc cd = p.chunks[c];
-        if (cd.nblk == 0) {
-            if (j == 0) {  // empty chunk: 7-byte header + EndMark
-                const uint32_t h = write_frame_header(cd.dst, 0);
-                cd.dst[h] = cd.dst[h + 1] = cd.dst[h + 2] = cd.dst[h + 3] = 0;
-                p.out_len[c] = h + 4;
-            }
-            continue;
-        }
-        if (j >= cd.nblk) continue;
-        const uint64_t boff = (uint64_t)j * kBlock;
-        d->src = cd.src + boff;
-        d->dst = cd.dst;
-        d->c = c;
-        d->j = j;
-        d->L = (uint32_t)min((uint64_t)kBlock, cd.len - boff);
-        d->last = (j + 1 == cd.nblk);
-        d->valid = 1;
-        if (j == 0) write_frame_header(cd.dst, cd.len);
-        return;
-    }
-}
-
 // Fused LZ4-frame + MD5 kernel.  Grid = 2 CTAs per SM, kWarps warps each.
 //   digest CTAs (blockIdx < n_md5_ctas): warps 0..3 each carry one MD5 group (32 chunks, lane = chunk, md5.cuh) at a time;
 //       when the groups are done the CTA joins the compressors.
 //   compressor CTAs: one 64 KiB block at a time -- bulk-load it into shared memory, warp 0 probes, warps 1.. parse
 //       (lz4.cuh), warp 0 plans the block's layout and takes its frame offset from the OFF chain, all warps write it out.
-// OFF chain (per chunk): (next block index << 40) | frame offset of that block -- a prefix sum handed from block j-1 to
-// block j as soon as j-1 knows its compressed size.  Waiting is deadlock-free: a CTA only waits on lower-numbered work
-// items, all of which were claimed earlier by running CTAs.
 __global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -250,13 +162,7 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) 
         if (warp < kProbers) {
             // ---------------------------------------------------------------- probers (warps 0 and 1, alternate batches of every segment)
             if (warp == 0) {
-                if (lane == 0) {
-                    const uint32_t bytes = (L + 15u) & ~15u;  // (the input slab is readable up to the next multiple of 16)
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic reads of the old block before the async write
-                    mbar_arrive_expect_tx(&ctl->in_full, bytes);
-                    for (uint32_t o = 0; o < bytes; o += kLoadPiece)  // several copies in flight: the pieces stream in parallel
-                        bulk_load(in + o, src + o, min(kLoadPiece, bytes - o), &ctl->in_full);
-                }
+                if (lane == 0) load_block(in, src, L, &ctl->in_full);
                 // clear the table meanwhile: entry 0 = (position 0, tag 0) doubles as "empty".  (Warp 1's first table access
                 // follows warp 0's first table phase through the token, so it sees the cleared table.)
                 uint4 *t4 = reinterpret_cast<uint4 *>(tab);
@@ -426,45 +332,20 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) 
                 }
                 csize = total + 1 + last + (last >= 15 ? (last - 15) / 255 + 1 : 0);
             }
-            const bool raw = csize > L - 1;  // LZ4F_makeBlock: a block that does not shrink is stored
-            // OFF chain: learn where this block starts, tell the successor at once
-            uint64_t st = 0;
             if (lane == 0) {
-                uint64_t *cw = p.chain + dsc->c;
-                unsigned ns = 128;
-                while (((st = ld_acquire(cw)) >> kOffBits) != dsc->j) {
-                    __nanosleep(ns);
-                    if (ns < 2048) ns <<= 1;
-                }
-                const uint64_t off = st & kOffMask;
-                const uint32_t bsize = raw ? L : csize;
-                const uint64_t end = off + 4 + bsize;
-                if (!dsc->last) st_release(p.chain + dsc->c, ((uint64_t)(dsc->j + 1) << kOffBits) | end);
-                uint8_t *hdr = dsc->dst + off;
-                const uint32_t hword = raw ? (L | 0x80000000u) : csize;
-                hdr[0] = (uint8_t)hword; hdr[1] = (uint8_t)(hword >> 8); hdr[2] = (uint8_t)(hword >> 16); hdr[3] = (uint8_t)(hword >> 24);
-                if (dsc->last) {
-                    uint8_t *e = dsc->dst + end;
-                    e[0] = e[1] = e[2] = e[3] = 0;  // EndMark
-                    p.out_len[dsc->c] = end + 4;
-                }
-                ctl->csize = csize;
-                ctl->raw = raw;
-                const uint64_t data = off + 4;
-                ctl->data_hi = (uint32_t)(data >> 32);
-                ctl->data_lo = (uint32_t)data;
+                const BlockPlace pl = place_block(p, *dsc, csize, L);
+                ctl->raw = pl.raw;
+                ctl->data = pl.data;
             }
         }
         __syncthreads();
 
         // ---------------------------------------------------------------- write the block to its final place (all warps)
         {
-            uint8_t *out = dsc->dst + (((uint64_t)ctl->data_hi << 32) | ctl->data_lo);
+            uint8_t *out = dsc->dst + ctl->data;
             if (ctl->raw) {
-                // stored block: straight from the input (L2-hot: the bulk load just pulled it), 16-byte-aligned slices per warp
-                const uint32_t per = (((L + kWarps - 1) / kWarps) + 15u) & ~15u;
-                const uint32_t lo = warp * per;
-                if (lo < L) warp_copy_stream<true>(out + lo, src + lo, min(per, L - lo), lane);
+                // stored block: straight from the input (L2-hot: the bulk load just pulled it)
+                copy_block<kWarps, true>(out, src, L, warp, lane);
             } else {
                 for (uint32_t s = warp; s < nseg; s += kWarps) {
                     const SegRec r = recs[s];
@@ -622,8 +503,6 @@ __global__ void sky_box_setup_kernel(BoxChunk *bc, uint64_t *blk_base, const Chu
 }
 
 }  // namespace sky
-
-#include "lz4hc.cuh"
 
 // ======================================================================================= host side
 using namespace sky;
@@ -894,7 +773,7 @@ uint32_t sky_kernel_config(int what) {
 
 uint64_t sky_frame_bound(uint64_t n) {
     if (n == 0) return 11;
-    return 15 + n + 4 * ((n + kBlock - 1) / kBlock) + 4;
+    return kFrameHeaderBytes + n + 4 * ((n + kBlock - 1) / kBlock) + 4;
 }
 
 static uint64_t round16(uint64_t x) { return (x + 15) & ~15ull; }
@@ -1048,7 +927,7 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
     uint32_t rows;
     int rc = batch_geometry(n, src_len, rows, [&](uint32_t i, uint32_t nblk) {
         m.h_desc[i] = ChunkDesc{d_src + src_off[i], d_dst + dst_off[i], src_len[i], nblk};
-        m.h_chain[i] = 15;  // block 0 starts right after the 15-byte frame header
+        m.h_chain[i] = kFrameHeaderBytes;  // OFF word: block 0 starts right after the frame header
     });
     if (rc != SKY_OK) return rc;
     const uint32_t ng = fill_md5_order(m.h_order, n, src_len);
