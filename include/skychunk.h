@@ -17,7 +17,9 @@
  * Output format: one LZ4 frame per chunk that lz4.frame.decompress (gateway_receiver.py:196)
  * restores bit-exactly: magic, FLG=0x68 (v01, independent blocks, content size), BD=0x40 (64 KiB),
  * u64le content size, header checksum, blocks (bit 31 set = stored raw), EndMark.  A zero-length
- * chunk yields the 11-byte frame liblz4 itself emits (content size omitted).
+ * chunk yields the 11-byte frame liblz4 itself emits (content size omitted).  With SKY_F_CHECKSUM the
+ * frame also carries LZ4's content checksum (FLG=0x6C, u32le XXH32 of the chunk after the EndMark).
+ * The receiver accepts block and content checksums in any frame and verifies them (SKY_D_CHECKSUM).
  */
 #ifndef SKYCHUNK_H
 #define SKYCHUNK_H
@@ -62,6 +64,14 @@ extern "C" {
  * LZ4 + MD5 + HC, as 0 means LZ4 + MD5; with stage bits it needs SKY_F_LZ4 (SKY_F_MD5 | SKY_F_HC is SKY_E_INVALID).
  * The digests come from the fused kernel's MD5-only mode running beside the HC kernel (two launches per batch). */
 #define SKY_F_HC 32u
+/* content checksum (sky_submit, with or without SKY_F_HC / SKY_F_E2EE, and sky_process_device): the frame carries
+ * XXH32(chunk, seed 0) as LZ4's content checksum, so any LZ4 decoder (lz4.frame.decompress, liblz4) verifies that it
+ * restores the chunk's bytes.  FLG becomes 0x6C (0x64 for an empty chunk, a 15-byte frame) and the frame ends with the
+ * EndMark followed by u32le XXH32; out_len includes those 4 bytes, and dst_cap[i] >= sky_frame_bound(src_len[i]) + 4
+ * (sky_box_bound(src_len[i]) + 4 with SKY_F_E2EE).  Alone it means LZ4 + MD5 + checksum; the MD5 lanes compute the
+ * XXH32, so the digests always come back; without SKY_F_LZ4 (no frame to carry it) it is SKY_E_INVALID.  One more launch
+ * per batch writes the checksums into the frames. */
+#define SKY_F_CHECKSUM 64u
 
 typedef struct sky_ctx sky_ctx;
 
@@ -125,7 +135,8 @@ SKY_API int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, cons
  * Replaces lz4.frame.decompress(to_write) (skyplane/gateway/operators/gateway_receiver.py:195-201) and supplies
  * the digest for the "# todo check hash" at gateway_receiver.py:231.  raw_len[i] is the expected decoded size
  * (WireProtocolHeader.raw_data_len, skyplane/chunk.py:100).  Accepts the frames this library emits (independent
- * 64 KiB blocks) and the reference sender's (linked blocks); status[i] = 0 or a SKY_D_* code (a bad frame is an
+ * 64 KiB blocks) and the reference sender's (linked blocks), with or without block and content checksums, which are
+ * verified; status[i] = 0 or a SKY_D_* code (a bad frame is an
  * error status, never a crash); md5[16*i..] = MD5 of the decoded bytes.
  * sky_decode_device: frames and output already in HBM (out_off multiples of 16; each frame region must be readable
  * up to the next multiple of 4 bytes, each output region writable up to the next multiple of 16).  sky_decode: host
@@ -140,6 +151,7 @@ SKY_API int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, cons
 #define SKY_D_LAYOUT (-5)
 #define SKY_D_TRUNCATED (-6)
 #define SKY_D_AUTH (-7) /* SKY_F_E2EE: the box's Poly1305 tag does not verify (nacl.exceptions.CryptoError in the reference) */
+#define SKY_D_CHECKSUM (-8) /* a block checksum or the content checksum (XXH32) does not match: lz4.frame.decompress raises */
 SKY_API int sky_decode_device(sky_ctx *ctx, uint32_t n, const void *d_frames, const uint64_t *frame_off, const uint64_t *frame_len,
                       void *d_out, const uint64_t *out_off, const uint64_t *raw_len, void *stream, int32_t *status, uint8_t *md5,
                       float *kernel_ms);

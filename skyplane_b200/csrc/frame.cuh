@@ -36,6 +36,7 @@ struct Params {
     uint32_t n_md5_ctas;        // CTAs 0..n_md5_ctas-1 digest (4 groups each at a time) before they compress
     uint32_t rows;  // max(1, max nblk)
     uint32_t flags;
+    uint32_t *xxh_out;          // per chunk XXH32 of the input (sky_fused_xxh_kernel only)
 };
 
 struct BlockDesc {            // written by the claiming thread, read by every warp after the block-start barrier

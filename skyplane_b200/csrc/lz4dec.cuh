@@ -3,10 +3,13 @@
 // Replaces lz4.frame.decompress(to_write) at skyplane/gateway/operators/gateway_receiver.py:195-201.
 // Two device steps:
 //   frame_index : one lane per chunk checks the frame header (magic, FLG, BD, content size, header checksum)
-//                 and walks the block headers, producing a block table (offset, size word) per chunk;
+//                 and walks the block headers, producing a block table (offset, size word, block checksum) per
+//                 chunk, and takes the content checksum from behind the EndMark;
 //   block decode: one warp per 64 KiB block.  Frames whose blocks are independent (what the H100 sender
 //                 emits) decode fully in parallel; linked-block frames (what the reference's CPU sender emits)
 //                 decode block j after block j-1 of the same chunk (matches may reach into earlier output).
+//                 A block checksum is verified before the block is decoded, as liblz4 does; the content checksum
+//                 by the MD5 lanes, which hash every decoded byte anyway (md5_warp<true>).
 // Every read and write is bounds-checked: a malformed frame yields an error status, never an out-of-range access.
 // The decoded size of block j is taken to be min(64 KiB, raw_len - j*64 KiB) -- true for liblz4 and for our
 // encoder (only the last block is short); anything else is reported as SKY_D_LAYOUT.
@@ -14,6 +17,7 @@
 #include <stdint.h>
 
 #include "lz4.cuh"
+#include "xxh32.cuh"
 
 namespace sky {
 
@@ -21,9 +25,12 @@ constexpr int32_t kDecOk = 0;
 constexpr int32_t kDecBadHeader = -1;   // magic / version / reserved bits / block size id / header checksum
 constexpr int32_t kDecCorrupt = -2;     // malformed sequence, offset out of range, overrun
 constexpr int32_t kDecSize = -3;        // content size or decoded size differs from the expected raw length
-constexpr int32_t kDecUnsupported = -4; // dictID / checksummed frames (never produced on this path)
+constexpr int32_t kDecUnsupported = -4; // dictID frames
 constexpr int32_t kDecLayout = -5;      // block structure does not match 64 KiB blocks with a short last one
-constexpr int32_t kDecTruncated = -6;   // frame ends inside a header or block
+constexpr int32_t kDecTruncated = -6;   // frame ends inside a header, block, checksum or before the content checksum
+constexpr int32_t kDecChecksum = -8;    // a block checksum or the content checksum does not match (-7 is SKY_D_AUTH)
+
+constexpr uint32_t kChkBlock = 1, kChkContent = 2;  // DecChunk::checks
 
 struct DecChunk {
     const uint8_t *frame;  // frame bytes (any alignment)
@@ -33,12 +40,14 @@ struct DecChunk {
     uint64_t blk_base;     // index of this chunk's first entry in the block table
     uint32_t nblk;
     uint32_t linked;       // written by frame_index: 1 = blocks may reference earlier blocks
+    uint32_t checks;       // written by frame_index for a well-formed frame: kChkBlock | kChkContent as FLG carries them
+    uint32_t content_xxh;  // written by frame_index: the frame's content checksum (kChkContent)
 };
 
 struct DecBlock {
     uint64_t off;    // offset of the block's data inside the frame
     uint32_t word;   // block header word (bit 31 = stored raw)
-    uint32_t pad;
+    uint32_t chk;    // the block's checksum, XXH32 of its stored bytes (kChkBlock)
 };
 
 __device__ __forceinline__ uint32_t rd32(const uint8_t *p) {
@@ -55,8 +64,8 @@ __device__ __forceinline__ void frame_index(DecChunk &cd, DecBlock *tbl, int32_t
     const uint8_t flg = f[4], bd = f[5];
     if ((flg >> 6) != 1 || (flg & 0x02) || (bd & 0x8F)) return fail(kDecBadHeader);
     if (((bd >> 4) & 7) != 4) return fail(((bd >> 4) & 7) < 4 ? kDecBadHeader : kDecLayout);  // 64 KiB blocks only
-    if (flg & 0x15) return fail(kDecUnsupported);  // block checksum / content checksum / dictID
-    const bool has_size = flg & 0x08;
+    if (flg & 0x01) return fail(kDecUnsupported);  // dictID
+    const bool has_size = flg & 0x08, block_chk = flg & 0x10, content_chk = flg & 0x04;
     const uint32_t hdr = 4 + 2 + (has_size ? 8 : 0) + 1;
     if (n < hdr + 4) return fail(kDecTruncated);
     uint8_t d[10];
@@ -79,11 +88,22 @@ __device__ __forceinline__ void frame_index(DecChunk &cd, DecBlock *tbl, int32_t
         if (n - ip < sz) return fail(kDecTruncated);
         tbl[j].off = ip;
         tbl[j].word = w;
-        tbl[j].pad = 0;
+        tbl[j].chk = 0;
         ip += sz;
+        if (block_chk) {
+            if (n - ip < 4) return fail(kDecTruncated);
+            tbl[j].chk = rd32(f + ip);
+            ip += 4;
+        }
     }
     if (n - ip < 4) return fail(kDecTruncated);
     if (rd32(f + ip) != 0) return fail(kDecSize);  // more blocks than the expected raw length allows
+    ip += 4;
+    if (content_chk) {
+        if (n - ip < 4) return fail(kDecTruncated);
+        cd.content_xxh = rd32(f + ip);
+    }
+    cd.checks = (block_chk ? kChkBlock : 0u) | (content_chk ? kChkContent : 0u);
 }
 
 // Copy `n` bytes from `op - offset` to `op` (LZ4 match semantics: the source may overlap the destination).

@@ -10,7 +10,7 @@
 // chain (ring of SKY_MD5_SLOTS x 64 B per lane, laid out [slot][piece][lane] so LDS.128 is conflict-free).
 #pragma once
 #include <stdint.h>
-
+#include "xxh32.cuh"
 #include <type_traits>
 #include <utility>
 
@@ -179,18 +179,21 @@ __device__ __forceinline__ void md5_unroll(F &&f) {
     md5_unroll_(f, std::make_integer_sequence<int, N>());
 }
 
+// md5_warp<true> also runs XXH32 (the LZ4 content checksum) over the same words: one 16-byte stripe after each MD5 round,
+// where its four short chains fill issue slots the MD5 chain leaves idle.
 // Digest of one chunk per lane.  `ring` = this warp's 8 KiB shared-memory area (2048 x uint32),
 // `src` 16-byte aligned (or len == 0), `active` false for lanes without a chunk.
-// Writes 16 digest bytes to `out` for active lanes.
+// Writes 16 digest bytes to `out` for active lanes.  kXxh: also returns XXH32(chunk, seed 0) (0 without kXxh or when
+// the lane is inactive).
 // `gate(row, wants)`: called (warp-converged) before the first byte of 64 KiB row `row` is fetched; `wants` tells
 // whether this lane has data in that row.  The receiver side uses it to wait until the row has been decoded.
 struct Md5NoGate {
     __device__ __forceinline__ void operator()(uint64_t, bool) const {}
 };
 
-template <class Gate = Md5NoGate>
-__device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uint64_t len, bool active, uint8_t *out,
-                                         unsigned lane, Gate gate = Gate()) {
+template <bool kXxh = false, class Gate = Md5NoGate>
+__device__ __forceinline__ uint32_t md5_warp(uint32_t *ring, const uint8_t *src, uint64_t len, bool active, uint8_t *out,
+                                             unsigned lane, Gate gate = Gate()) {
     constexpr int kSlots = SKY_MD5_SLOTS;  // ring depth (blocks, power of two); prefetch distance = kSlots - 1
     static_assert(kSlots >= 2 && (kSlots & (kSlots - 1)) == 0 && 1024 % kSlots == 0, "SKY_MD5_SLOTS: a power of two, 2..1024");
     constexpr bool kGated = !std::is_same<Gate, Md5NoGate>::value;
@@ -202,6 +205,11 @@ __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uin
     Md5State st;  // runs on through the blocks past this lane's end (the loop has no branch per lane) ...
     md5_init(st);
     Md5State fin = st;  // ... so the state after the lane's last full block is kept here, off the chain
+    XxhState xs, xfin;  // (kXxh) the same for the XXH32 accumulators
+    if constexpr (kXxh) {
+        xxh_init(xs);
+        xfin = xs;
+    }
     // slot s, piece q of this lane lives at ring[((s*4 + q)*32 + lane) * 4 words]: a per-lane base plus an immediate
     const uint32_t *lring = ring + lane * 4;
     const uint32_t lring_s = (uint32_t)__cvta_generic_to_shared(lring);
@@ -238,19 +246,30 @@ __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uin
             constexpr int ps = (u + kSlots - 1) & (kSlots - 1);  // slot of block i+u-1, read during block i+u-2
             constexpr int ns = (u + 1) & (kSlots - 1);
             uint32_t a = st.a, b = st.b, c = st.c, d = st.d;
-            md5_round<0>(a, b, c, d, w[u & 1], one);
+            const uint32_t(&wu)[16] = w[u & 1];
+            auto stripe = [&](int q) {
+                if constexpr (kXxh) xxh_stripe(xs, wu[4 * q], wu[4 * q + 1], wu[4 * q + 2], wu[4 * q + 3]);
+            };
+            md5_round<0>(a, b, c, d, wu, one);
+            stripe(0);
             cp_async_block<ps>(i + u + (kSlots - 1) < nfull, lring_s, pf_src + u * 64);
-            md5_round<1>(a, b, c, d, w[u & 1], one);
+            md5_round<1>(a, b, c, d, wu, one);
+            stripe(1);
             cp_async_commit();
             cp_async_wait<kSlots - 2>();  // block i+u+1 has landed
-            md5_round<2>(a, b, c, d, w[u & 1], one);
+            md5_round<2>(a, b, c, d, wu, one);
+            stripe(2);
             load_words(w[(u + 1) & 1], ns);
-            md5_round<3>(a, b, c, d, w[u & 1], one);
+            md5_round<3>(a, b, c, d, wu, one);
+            stripe(3);
             st.a += a;
             st.b += b;
             st.c += c;
             st.d += d;
-            if (i + u < nfull) fin = st;
+            if (i + u < nfull) {
+                fin = st;
+                if constexpr (kXxh) xfin = xs;
+            }
         });
         pf_src += kSlots * 64;
     };
@@ -269,6 +288,7 @@ __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uin
     }
     cp_async_wait<0>();
     st = fin;
+    uint32_t xxh = 0;
     if (active) {
         // tail: rem bytes + 0x80 + zeros + u64le bit length -> one or two more blocks (slow path, once per chunk)
         const uint32_t rem = (uint32_t)(len & 63);
@@ -277,6 +297,16 @@ __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uin
 #pragma unroll
         for (int k = 0; k < 32; k++) tw[k] = 0;
         for (uint32_t k = 0; k < rem; k++) tw[k >> 2] |= (uint32_t)tp[k] << (8 * (k & 3));
+        if constexpr (kXxh) {
+            // XXH32 of the tail: its 0-3 whole stripes, then 4-byte words, then single bytes, then the avalanche
+            xs = xfin;
+            const uint32_t nstripes = rem >> 4;
+            for (uint32_t q = 0; q < nstripes; q++) xxh_stripe(xs, tw[4 * q], tw[4 * q + 1], tw[4 * q + 2], tw[4 * q + 3]);
+            uint32_t h = xxh_merge(xs, len);
+            for (uint32_t k = 4 * nstripes; k < (rem >> 2); k++) h = xxh_word(h, tw[k]);
+            for (uint32_t k = rem & ~3u; k < rem; k++) h = xxh_byte(h, (tw[k >> 2] >> (8 * (k & 3))) & 0xffu);
+            xxh = xxh_avalanche(h);
+        }
         tw[rem >> 2] |= 0x80u << (8 * (rem & 3));
         const bool two = rem >= 56;
         const uint64_t bits = len << 3;
@@ -291,6 +321,7 @@ __device__ __forceinline__ void md5_warp(uint32_t *ring, const uint8_t *src, uin
         uint4 dg = make_uint4(st.a, st.b, st.c, st.d);
         *reinterpret_cast<uint4 *>(out) = dg;  // out is 16-byte aligned (md5 array base is 256-aligned)
     }
+    return xxh;
 }
 
 }  // namespace sky

@@ -91,12 +91,13 @@ __device__ __forceinline__ void bar_arrive() { asm volatile("bar.arrive %0, 64;"
 template <int kId>
 __device__ __forceinline__ void bar_wait() { asm volatile("bar.sync %0, 64;" ::"n"(kId) : "memory"); }
 
-// Fused LZ4-frame + MD5 kernel.  Grid = 2 CTAs per SM, kWarps warps each.
+// Fused LZ4-frame + MD5 kernel body.  Grid = 2 CTAs per SM, kWarps warps each.
 //   digest CTAs (blockIdx < n_md5_ctas): warps 0..3 each carry one MD5 group (32 chunks, lane = chunk, md5.cuh) at a time;
-//       when the groups are done the CTA joins the compressors.
+//       when the groups are done the CTA joins the compressors.  kXxh: the MD5 lanes also write XXH32(chunk) to xxh_out.
 //   compressor CTAs: one 64 KiB block at a time -- bulk-load it into shared memory, warp 0 probes, warps 1.. parse
 //       (lz4.cuh), warp 0 plans the block's layout and takes its frame offset from the OFF chain, all warps write it out.
-__global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) {
+template <bool kXxh>
+__device__ __forceinline__ void fused_body(const Params &p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint8_t *in = smem + kInOff;
@@ -131,8 +132,11 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) 
                     src = p.chunks[c].src;
                     len = p.chunks[c].len;
                 }
-                md5_warp(reinterpret_cast<uint32_t *>(in + warp * kRingBytes), src, len, active, p.md5_out + (size_t)(active ? c : 0) * 16,
-                         lane);
+                const uint32_t x = md5_warp<kXxh>(reinterpret_cast<uint32_t *>(in + warp * kRingBytes), src, len, active,
+                                                  p.md5_out + (size_t)(active ? c : 0) * 16, lane);
+                if constexpr (kXxh) {
+                    if (active) p.xxh_out[c] = x;
+                }
                 __syncwarp();
             }
         }
@@ -366,6 +370,29 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) 
     }
 }
 
+__global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) { fused_body<false>(p); }
+// SKY_F_CHECKSUM: the same kernel with the content checksum computed by the MD5 lanes (sky_checksum_kernel writes it).
+__global__ void __launch_bounds__(kThreads, 2) sky_fused_xxh_kernel(const Params p) { fused_body<true>(p); }
+
+// SKY_F_CHECKSUM epilogue, one thread per chunk, after the compressor has finished the frame: FLG gains C.Checksum
+// (0x68 -> 0x6C, 0x60 -> 0x64 for an empty chunk), the header checksum byte follows, and the XXH32 of the chunk goes
+// behind the EndMark.
+__global__ void sky_checksum_kernel(const ChunkDesc *chunks, const uint32_t *xxh, uint64_t *out_len, uint32_t n) {
+    const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n) return;
+    const ChunkDesc cd = chunks[c];
+    uint8_t *f = cd.dst;
+    const uint32_t dlen = cd.len ? 10u : 2u;  // FLG, BD (+ content size)
+    f[4] |= 0x04;
+    uint8_t d[10];
+    for (uint32_t i = 0; i < dlen; i++) d[i] = f[4 + i];
+    f[4 + dlen] = (uint8_t)(xxh32_small(d, dlen) >> 8);
+    const uint64_t end = out_len[c];
+    const uint32_t x = xxh[c];
+    f[end] = (uint8_t)x; f[end + 1] = (uint8_t)(x >> 8); f[end + 2] = (uint8_t)(x >> 16); f[end + 3] = (uint8_t)(x >> 24);
+    out_len[c] = end + 4;
+}
+
 
 // ------------------------------------------------------------------------------------ receiver side
 struct DecParams {
@@ -389,6 +416,8 @@ __global__ void sky_frame_index_kernel(const DecParams p) {
     int32_t st = kDecOk;
     frame_index(cd, p.blocks + cd.blk_base, &st);
     p.chunks[c].linked = cd.linked;
+    p.chunks[c].checks = cd.checks;
+    p.chunks[c].content_xxh = cd.content_xxh;
     p.status[c] = st;
 }
 
@@ -410,7 +439,9 @@ struct DecRowGate {
 };
 
 // Persistent: warps 0..3 of a CTA may host an MD5 group (digest of the decoded bytes, following the decode through
-// per-block flags); every other warp (and MD5 warps once their groups are done) decodes blocks.
+// per-block flags); every other warp (and MD5 warps once their groups are done) decodes blocks.  The MD5 lanes always
+// compute the XXH32 of the decoded bytes too (whether a frame carries a content checksum is only known on the device)
+// and compare it where the frame has one.
 __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -427,8 +458,10 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
                 len = p.chunks[c].raw_len;
                 gate.flags = p.blk_done + p.chunks[c].blk_base;
             }
-            md5_warp(reinterpret_cast<uint32_t *>(smem + warp * kRingBytes), src, len, active, p.md5_out + (size_t)(active ? c : 0) * 16,
-                     lane, gate);
+            const uint32_t x = md5_warp<true>(reinterpret_cast<uint32_t *>(smem + warp * kRingBytes), src, len, active,
+                                              p.md5_out + (size_t)(active ? c : 0) * 16, lane, gate);
+            // every row has passed the gate, so the chunk's decode status is final: a checksum mismatch only replaces ok
+            if (active && (p.chunks[c].checks & kChkContent) && x != p.chunks[c].content_xxh) atomicCAS(p.status + c, kDecOk, kDecChecksum);
             __syncwarp();
         }
     }
@@ -458,7 +491,9 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
         if (st == kDecOk) {
             const DecBlock b = p.blocks[cd.blk_base + j];
             const uint32_t sz = b.word & 0x7FFFFFFFu;
-            if (b.word & 0x80000000u) {
+            if ((cd.checks & kChkBlock) && xxh32_warp(cd.frame + b.off, sz, lane) != b.chk) {
+                st = kDecChecksum;
+            } else if (b.word & 0x80000000u) {
                 if (sz != want) st = kDecLayout;
                 else warp_copy(cd.out + pos, cd.frame + b.off, sz, lane);
             } else {
@@ -547,6 +582,7 @@ struct BatchMeta {  // one batch's descriptors and results (the receiver uses th
     // device->host copies sit in a copy-engine queue behind multi-GiB frame copies
     Mapped<uint64_t> outlen;
     Mapped<uint8_t> md5;
+    DevMem<uint32_t> xxh;     // per chunk XXH32 of the input (SKY_F_CHECKSUM)
     DevMem<uint32_t> counters;
     DevMem<uint8_t> scratch;  // compress scratch: kScratchBytes per CTA of the grid (kernels of different slots overlap)
 };
@@ -648,6 +684,7 @@ static int build_slot(sky_ctx *ctx, Slot &s, bool slabs) {
     CK(ctx, cudaMalloc(m.d_chain.put(), nc * sizeof(uint64_t)));
     CK(ctx, m.outlen.alloc(nc));
     CK(ctx, m.md5.alloc(nc * 16));
+    CK(ctx, cudaMalloc(m.xxh.put(), nc * sizeof(uint32_t)));
     CK(ctx, cudaMalloc(m.counters.put(), 64));
     CK(ctx, cudaMalloc(m.scratch.put(), (size_t)ctx->sm_count * kCtasPerSm * kScratchBytes));
     if (slabs) {
@@ -788,13 +825,16 @@ int sky_ctx_create(int device, uint64_t max_batch_bytes, uint32_t max_chunks, ui
     if (!ctx) return SKY_E_NOMEM;
     ctx->device = device;
     ctx->max_chunks = max_chunks;
-    // every chunk is placed at a 16-byte aligned offset; frames need bound(len) each
+    // every chunk is placed at a 16-byte aligned offset; frames need bound(len) each (+ 4 with SKY_F_CHECKSUM), and a
+    // received frame with block checksums 4 more bytes per block
     ctx->in_cap = round16(max_batch_bytes) + 16ull * max_chunks + 256;
-    ctx->out_cap = max_batch_bytes + (uint64_t)max_chunks * (64 + 4 * 2) + 4 * (max_batch_bytes / kBlock + 1) + 256;
+    ctx->out_cap = max_batch_bytes + (uint64_t)max_chunks * (64 + 4 * 3) + 8 * (max_batch_bytes / kBlock + 1) + 256;
     CK(ctx, cudaSetDevice(device));
     CK(ctx, cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
     cudaError_t e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_xxh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_xxh_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_hc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
     if (e != cudaSuccess) {
         g_err = ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (this build carries sm_90a code only)";
@@ -910,8 +950,13 @@ static uint32_t fill_md5_order(uint32_t *order, uint32_t n, const uint64_t *len)
     return ng;
 }
 
-// SKY_F_HC selects how frames are made, so it needs SKY_F_LZ4, or no stage bit at all (= LZ4 + MD5).
-static bool hc_flags_valid(uint32_t flags) { return !(flags & SKY_F_HC) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5; }
+// SKY_F_HC selects how frames are made and SKY_F_CHECKSUM adds to the frame, so each needs SKY_F_LZ4, or no stage bit at
+// all (= LZ4 + MD5).
+static bool frame_flags_valid(uint32_t flags) {
+    return !(flags & (SKY_F_HC | SKY_F_CHECKSUM)) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5;
+}
+// Bytes a chunk's frame may take: SKY_F_CHECKSUM adds the 4-byte content checksum behind the EndMark.
+static uint64_t frame_need(uint64_t n, uint32_t flags) { return sky_frame_bound(n) + ((flags & SKY_F_CHECKSUM) ? 4 : 0); }
 
 // Fills the slot's metadata for a batch and enqueues: meta H2D, counter reset, fused kernel, results D2H.
 // `meta_st`: stream the three small metadata copies ride on (the H2D stream on the host path, so they are
@@ -919,6 +964,8 @@ static bool hc_flags_valid(uint32_t flags) { return !(flags & SKY_F_HC) || (flag
 static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t meta_st, uint32_t n, const uint8_t *d_src,
                         const uint64_t *src_off, const uint64_t *src_len, uint8_t *d_dst, const uint64_t *dst_off, uint32_t flags) {
     if ((flags & (SKY_F_LZ4 | SKY_F_MD5)) == 0) flags |= SKY_F_LZ4 | SKY_F_MD5;
+    if (flags & SKY_F_CHECKSUM) flags |= SKY_F_MD5;  // the content checksum comes from the MD5 lanes
+    const bool xxh = (flags & SKY_F_CHECKSUM) != 0;
     if (flags & SKY_F_HC) {
         const int hrc = alloc_hc(ctx, s.hc);
         if (hrc != SKY_OK) return hrc;
@@ -961,6 +1008,7 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
                                                                  std::min(ng, (uint32_t)ctx->sm_count / 4))) : 0;
     p.rows = rows;
     p.flags = flags;
+    p.xxh_out = m.xxh;
     CK(ctx, cudaEventRecord(s.ev_k0, st));
     if (flags & SKY_F_HC) {
         // high-ratio frames from sky_hc_kernel; the digests from the fused kernel's MD5-only mode on a forked stream, so
@@ -972,7 +1020,8 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
             CK(ctx, cudaStreamWaitEvent(h.md5_stream, h.ev_fork, 0));
             Params pm = p;
             pm.flags = SKY_F_MD5;
-            sky_fused_kernel<<<grid, kThreads, kSmemBytes, h.md5_stream>>>(pm);
+            if (xxh) sky_fused_xxh_kernel<<<grid, kThreads, kSmemBytes, h.md5_stream>>>(pm);
+            else sky_fused_kernel<<<grid, kThreads, kSmemBytes, h.md5_stream>>>(pm);
             CK(ctx, cudaGetLastError());
             CK(ctx, cudaEventRecord(h.ev_join, h.md5_stream));
             ctx->launches++;
@@ -982,11 +1031,17 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
         CK(ctx, cudaGetLastError());
         if (md5) CK(ctx, cudaStreamWaitEvent(st, h.ev_join, 0));
     } else {
-        sky_fused_kernel<<<grid, kThreads, kSmemBytes, st>>>(p);
+        if (xxh) sky_fused_xxh_kernel<<<grid, kThreads, kSmemBytes, st>>>(p);
+        else sky_fused_kernel<<<grid, kThreads, kSmemBytes, st>>>(p);
         CK(ctx, cudaGetLastError());
     }
-    CK(ctx, cudaEventRecord(s.ev_k1, st));
     ctx->launches++;
+    if (xxh) {
+        sky_checksum_kernel<<<(n + 127) / 128, 128, 0, st>>>(m.d_desc, m.xxh, m.outlen.d, n);
+        CK(ctx, cudaGetLastError());
+        ctx->launches++;
+    }
+    CK(ctx, cudaEventRecord(s.ev_k1, st));
     if (flags & SKY_F_E2EE) {
         rc = launch_seal(ctx, s, st, n, d_dst, flags);
         if (rc != SKY_OK) return rc;
@@ -1027,12 +1082,12 @@ int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64
                        uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
     if (!ctx || n == 0 || !src_off || !src_len || !dst_off || !dst_cap || !d_dst) return SKY_E_INVALID;
     if (flags & SKY_F_E2EE) return SKY_E_INVALID;  // boxes are a host-path feature (sky_submit)
-    if (!hc_flags_valid(flags)) return SKY_E_INVALID;
+    if (!frame_flags_valid(flags)) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
     if ((reinterpret_cast<uintptr_t>(d_src) & 15) || (reinterpret_cast<uintptr_t>(d_dst) & 15)) return SKY_E_INVALID;
     for (uint32_t i = 0; i < n; i++) {
         if ((src_off[i] & 15) || (dst_off[i] & 15)) return SKY_E_INVALID;
-        if (dst_cap[i] < sky_frame_bound(src_len[i])) return SKY_E_CAPACITY;
+        if (dst_cap[i] < frame_need(src_len[i], flags)) return SKY_E_CAPACITY;
         if (src_len[i] && !d_src) return SKY_E_INVALID;
     }
     CK(ctx, cudaSetDevice(ctx->device));
@@ -1050,7 +1105,7 @@ int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64
 
 int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t *src_len, void *const *dst,
                const uint64_t *dst_cap, uint32_t flags, const uint8_t *nonces, uint64_t *ticket) {
-    if (!ctx || n == 0 || !src || !src_len || !ticket || !hc_flags_valid(flags)) return SKY_E_INVALID;
+    if (!ctx || n == 0 || !src || !src_len || !ticket || !frame_flags_valid(flags)) return SKY_E_INVALID;
     if ((flags & (SKY_F_LZ4 | SKY_F_MD5)) == 0) flags |= SKY_F_LZ4 | SKY_F_MD5;
     const bool e2ee = (flags & SKY_F_E2EE) != 0, frames = (flags & SKY_F_LZ4) != 0;
     const bool returns_data = frames || e2ee;  // MD5-only without E2EE: only digests come back
@@ -1069,13 +1124,13 @@ int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t 
     for (uint32_t i = 0; i < n; i++) {
         if (src_len[i] && !src[i]) return SKY_E_INVALID;
         if (returns_data) {
-            const uint64_t need = (frames ? sky_frame_bound(src_len[i]) : src_len[i]) + (e2ee ? kBoxOverhead : 0);
+            const uint64_t need = (frames ? frame_need(src_len[i], flags) : src_len[i]) + (e2ee ? kBoxOverhead : 0);
             if (!dst[i] || dst_cap[i] < need) return SKY_E_CAPACITY;
         }
         in_off[i] = ip;
         out_off[i] = op;
         ip += round16(src_len[i]);
-        op += round16(sky_frame_bound(src_len[i]));
+        op += round16(frame_need(src_len[i], flags));
     }
     if (ip > ctx->in_cap || op > ctx->out_cap) return SKY_E_CAPACITY;
     for (uint32_t i = 0; i < n; i++)

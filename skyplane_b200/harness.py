@@ -56,11 +56,13 @@ def run_stream(
     operator_cls=GatewayCompressHash,
     n_slots: int = 4,
     high_ratio: bool = False,
+    content_checksum: bool = False,
 ) -> Dict:
     """Stream ``n_requests`` chunk requests (recycling ``pool_files`` by hard link) through the operator.
 
     The first ``warmup_requests`` completions are not timed (worker start-up: CUDA context, pinned staging).
-    ``high_ratio`` is handed to the operator (GatewayCompressHash's high-ratio frames) when set.
+    ``high_ratio`` and ``content_checksum`` are handed to the operator (GatewayCompressHash's high-ratio frames, frames with
+    LZ4's content checksum) when set.
     Returns {"wall_s", "bytes", "records": [{chunk_id, pool_index, md5, raw_len, frame_path}], "status": {...}}.
     """
     chunk_dir = Path(chunk_dir)
@@ -72,6 +74,7 @@ def run_stream(
         "compress_hash", "local:box", qin, qout, err_ev, err_q, store, n_processes=n_workers,
         max_batch_chunks=max_batch_chunks, max_batch_bytes=max_batch_bytes, n_gpus=n_gpus, keep_frames_on_disk=keep_frames, n_slots=n_slots,
         **({"high_ratio": True} if high_ratio else {}),
+        **({"content_checksum": True} if content_checksum else {}),
     )
     op.start_workers()
     records: List[Dict] = []

@@ -14,12 +14,13 @@ LIB_PATH = _PKG / "libskychunk.so"
 
 SKY_OK = 0
 SKY_E_INVALID, SKY_E_NOGPU, SKY_E_CUDA, SKY_E_CAPACITY, SKY_E_BUSY, SKY_E_TICKET, SKY_E_NOMEM, SKY_E_NOKEY = -1, -2, -3, -4, -5, -6, -7, -8
-F_LZ4, F_MD5, F_E2EE, F_HC = 1, 2, 16, 32
+F_LZ4, F_MD5, F_E2EE, F_HC, F_CHECKSUM = 1, 2, 16, 32, 64
+CHECKSUM_BYTES = 4  # F_CHECKSUM: the content checksum (u32le XXH32) behind the EndMark
 BOX_OVERHEAD = 40
 # sky_decode status codes
-D_OK, D_BAD_HEADER, D_CORRUPT, D_SIZE, D_UNSUPPORTED, D_LAYOUT, D_TRUNCATED, D_AUTH = 0, -1, -2, -3, -4, -5, -6, -7
+D_OK, D_BAD_HEADER, D_CORRUPT, D_SIZE, D_UNSUPPORTED, D_LAYOUT, D_TRUNCATED, D_AUTH, D_CHECKSUM = 0, -1, -2, -3, -4, -5, -6, -7, -8
 D_NAMES = {0: "ok", -1: "bad frame header", -2: "corrupt block", -3: "size mismatch", -4: "unsupported frame feature",
-           -5: "unexpected block layout", -6: "truncated frame", -7: "box authentication failed"}
+           -5: "unexpected block layout", -6: "truncated frame", -7: "box authentication failed", -8: "checksum mismatch"}
 
 # every symbol include/skychunk.h declares (tests check the .so exports exactly these)
 ABI_SYMBOLS = (

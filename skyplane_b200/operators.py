@@ -134,12 +134,16 @@ class GatewayCompressHash(GatewayOperator):
         sink=None,
         n_slots: int = 4,
         high_ratio: bool = False,
+        content_checksum: bool = False,
     ):
         """use_compression / e2ee_key_bytes: GatewaySender's arguments of the same name (gateway_operator.py:154-168):
         ``use_compression=False`` digests the chunk and lets it pass through uncompressed (``is_compressed=False``);
         ``e2ee_key_bytes`` seals every payload in a SecretBox on the GPU.
         high_ratio: frames from the high-ratio parse (``ChunkStage.launch(hc=True)``): same frame format and receiver,
         fewer bytes on the wire for more GPU time per chunk.  Needs ``use_compression``.
+        content_checksum: every frame carries LZ4's content checksum (XXH32 of the chunk, python-lz4's argument of the same
+        name), so any receiver that decodes it with ``lz4.frame.decompress`` verifies the chunk's bytes end to end; the GPU
+        receiver verifies it too.  Needs ``use_compression``.
         sink: ``callable(worker_id) -> socket``, called once in each worker.  With a sink the worker sends every payload
         straight from the pinned staging slot (``wire.send_results``: WireProtocolHeader + payload, no intermediate bytes
         object, no frame file) -- the tail of ``GatewaySender.process`` (gateway_operator.py:367-402)."""
@@ -148,6 +152,9 @@ class GatewayCompressHash(GatewayOperator):
         if high_ratio and not self.use_compression:
             raise ValueError("high_ratio selects how chunks are compressed: it needs use_compression")
         self.high_ratio = bool(high_ratio)
+        if content_checksum and not self.use_compression:
+            raise ValueError("content_checksum is carried by the LZ4 frame: it needs use_compression")
+        self.content_checksum = bool(content_checksum)
         self.e2ee_key_bytes = e2ee_key_bytes
         self.sink = sink
         # batches in flight per worker: a batch of 8 MiB chunks spends >= 70 ms on the GPU whatever its size (one serial MD5
@@ -290,10 +297,10 @@ class GatewayCompressHash(GatewayOperator):
         if not all([fut.result() for _, fut in jobs]):
             stage.release(slot)
             return False
-        if self.high_ratio:
-            stage.launch(slot, compress=True, encrypt=self.e2ee_key_bytes is not None, hc=True)
-        else:
-            stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None)
+        opts = {"hc": True} if self.high_ratio else {}
+        if self.content_checksum:
+            opts["checksum"] = True
+        stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None, **opts)
         return True
 
     def _launch(self, reqs: List[ChunkRequest]):
@@ -419,7 +426,8 @@ class GatewayCompressHash(GatewayOperator):
 
 
 class ChecksumMismatchException(Exception):
-    """Same name as skyplane/exceptions.py:44-48: the decoded chunk's MD5 differs from Chunk.md5_hash."""
+    """Same name as skyplane/exceptions.py:44-48: the decoded chunk's MD5 differs from Chunk.md5_hash, or the frame's own
+    block or content checksum (XXH32) does not match."""
 
 
 class GatewayDecompressVerify(GatewayOperator):
@@ -500,6 +508,8 @@ class GatewayDecompressVerify(GatewayOperator):
             chunk = reqs[i].chunk
             if status in (native.D_TRUNCATED, native.D_BAD_HEADER, native.D_AUTH) and self._still_arriving(chunk.chunk_id, len(frame)):
                 continue  # a writer may still be appending (a short box fails authentication, a short frame is truncated)
+            if status == native.D_CHECKSUM:  # complete frame whose block or content checksum fails: never "still arriving"
+                raise ChecksumMismatchException(f"chunk {chunk.chunk_id}: LZ4 frame checksum does not match the decoded bytes")
             if status != 0:
                 raise ValueError(f"chunk {chunk.chunk_id}: payload rejected ({native.D_NAMES.get(status, status)})")
             want = chunk.md5_hash

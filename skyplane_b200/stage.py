@@ -35,6 +35,12 @@ class StageResult:
         return bytes(self.frame)
 
 
+def _out_room(n: int) -> int:
+    """Staging bytes an n-byte chunk's payload may take: its frame with the content checksum (launch(checksum=True)),
+    sealed in a SecretBox (encrypt=True).  Reserved whatever the batch is launched with."""
+    return native.round16(native.frame_bound(n) + native.CHECKSUM_BYTES + native.BOX_OVERHEAD)
+
+
 class _Slot:
     def __init__(self, in_bytes: int, out_bytes: int):
         self.inp = native.PinnedBuffer(in_bytes)
@@ -52,15 +58,15 @@ class _Slot:
 
     def reserve(self, n: int) -> memoryview:
         """Reserve room for an n-byte chunk; returns the writable pinned view to fill."""
-        bound = native.frame_bound(n) + native.BOX_OVERHEAD  # (room for the SecretBox nonce + tag when E2EE is on)
-        if self.in_used + native.round16(n) > self.inp.nbytes or self.out_used + native.round16(bound) > self.out.nbytes:
+        room = _out_room(n)
+        if self.in_used + native.round16(n) > self.inp.nbytes or self.out_used + room > self.out.nbytes:
             raise native.SkyChunkError(native.SKY_E_CAPACITY, "batch exceeds the stage's staging buffers")
         off = self.in_used
         self.in_off.append(off)
         self.lens.append(n)
         self.out_off.append(self.out_used)
         self.in_used += native.round16(n)
-        self.out_used += native.round16(bound)
+        self.out_used += room
         return self.inp.view[off : off + n]
 
 
@@ -94,7 +100,7 @@ class ChunkStage:
         return (
             len(slot.lens) < self.max_chunks
             and slot.in_used + native.round16(n) <= slot.inp.nbytes
-            and slot.out_used + native.round16(native.frame_bound(n) + native.BOX_OVERHEAD) <= slot.out.nbytes
+            and slot.out_used + _out_room(n) <= slot.out.nbytes
         )
 
     def add_bytes(self, slot: _Slot, data: BytesLike) -> int:
@@ -141,7 +147,7 @@ class ChunkStage:
         if got != length:
             slot.in_off.pop(); slot.lens.pop(); slot.out_off.pop()
             slot.in_used -= native.round16(length)
-            slot.out_used -= native.round16(native.frame_bound(length) + native.BOX_OVERHEAD)
+            slot.out_used -= _out_room(length)
             raise EOFError(f"stream ended after {got} of {length} bytes")
         return len(slot.lens) - 1
 
@@ -150,24 +156,30 @@ class ChunkStage:
         self.ctx.set_e2ee_key(key)
         self._has_key = key is not None
 
-    def launch(self, slot: _Slot, compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None, hc: bool = False) -> _Slot:
+    def launch(self, slot: _Slot, compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None, hc: bool = False,
+               checksum: bool = False) -> _Slot:
         """compress=False is the reference's `compress: false` (digest only, the chunk passes through);
         encrypt=True seals every payload with the stage's key (nonces: 24 bytes per chunk, default os.urandom);
-        hc=True makes the frames with the high-ratio parse (F_HC): same frame format, fewer bytes, more GPU time."""
+        hc=True makes the frames with the high-ratio parse (F_HC): same frame format, fewer bytes, more GPU time;
+        checksum=True gives every frame LZ4's content checksum (F_CHECKSUM), which any LZ4 decoder verifies."""
         if not slot.lens:
             raise ValueError("empty batch")
         if hc and not compress:
             raise ValueError("hc=True selects how frames are compressed: it needs compress=True")
+        if checksum and not compress:
+            raise ValueError("checksum=True is carried by the LZ4 frame: it needs compress=True")
         if hc and not native.kernel_config()["hc_depth"]:
             raise native.SkyChunkError(native.SKY_E_INVALID, f"{native.LIB_PATH.name} was built without the high-ratio kernel (F_HC)")
         base_in, base_out = slot.inp.addr, slot.out.addr
         src = [base_in + o for o in slot.in_off]
-        flags = native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0) | (native.F_HC if hc else 0)
+        flags = (native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0) | (native.F_HC if hc else 0)
+                 | (native.F_CHECKSUM if checksum else 0))
         if encrypt and nonces is None:
             nonces = os.urandom(24 * len(slot.lens))  # what nacl.utils.random(24) draws per message
         if compress or encrypt:
             dst = [base_out + o for o in slot.out_off]
-            caps = [(native.frame_bound(n) if compress else n) + (native.BOX_OVERHEAD if encrypt else 0) for n in slot.lens]
+            caps = [(native.frame_bound(n) + (native.CHECKSUM_BYTES if checksum else 0) if compress else n)
+                    + (native.BOX_OVERHEAD if encrypt else 0) for n in slot.lens]
         else:
             dst = caps = None
         slot.flags = flags
@@ -187,8 +199,9 @@ class ChunkStage:
 
     # ------------------------------------------------------------------ sync convenience
     def process(self, chunks: Sequence[BytesLike], compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None,
-                hc: bool = False) -> List[StageResult]:
-        """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes (hc: see launch)."""
+                hc: bool = False, checksum: bool = False) -> List[StageResult]:
+        """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes (hc, checksum:
+        see launch)."""
         out: List[StageResult] = []
         i = 0
         while i < len(chunks):
@@ -200,7 +213,7 @@ class ChunkStage:
             if j == i:
                 self.release(slot)
                 raise native.SkyChunkError(native.SKY_E_CAPACITY, f"chunk of {memoryview(chunks[i]).nbytes} bytes exceeds max_batch_bytes")
-            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc)
+            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum)
             for r in self.collect(slot):
                 out.append(StageResult(frame=memoryview(bytes(r.frame)), md5=r.md5, raw_len=r.raw_len, comp_len=r.comp_len,
                                        is_compressed=r.is_compressed, is_encrypted=r.is_encrypted))

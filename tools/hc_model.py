@@ -51,9 +51,9 @@ def frame(data: bytes, o: Opts | None = None) -> bytes:
     return tile_model.assemble(len(data), blocks(data, o or kernel_opts()))
 
 
-def liblz4_frame(data: bytes, level: int, linked: bool = False) -> bytes:
+def liblz4_frame(data: bytes, level: int, linked: bool = False, content_checksum: bool = False, block_checksum: bool = False) -> bytes:
     """liblz4's frame at compression `level` (>= 3: its HC search), 64 KiB blocks, independent unless `linked` -- what the
-    high-ratio mode is compared with."""
+    high-ratio mode is compared with; with LZ4's content / block checksums (XXH32) when asked for."""
     import oracle.reflib as ref
 
     L = ref._lib()
@@ -61,6 +61,8 @@ def liblz4_frame(data: bytes, level: int, linked: bool = False) -> bytes:
     prefs = ref._prefs(n)
     prefs.compressionLevel = level
     prefs.frameInfo.blockMode = 0 if linked else 1
+    prefs.frameInfo.contentChecksumFlag = int(content_checksum)
+    prefs.frameInfo.blockChecksumFlag = int(block_checksum)
     cap = L.LZ4F_compressFrameBound(n, ctypes.byref(prefs))
     out = ctypes.create_string_buffer(cap)
     r = L.LZ4F_compressFrame(ctypes.cast(out, ctypes.c_void_p), cap, ptr, n, ctypes.byref(prefs))

@@ -2,9 +2,10 @@
 
 On sm_90a the integer ops of the MD5 chain have fixed latency, so ptxas schedules them by the stall count it writes into
 each instruction's control bits (bits 41-44 of the high 64-bit word).  With no variable-latency op on the chain, the sum
-of the stall counts over the loop is the loop's time in cycles.  For `sky_fused_kernel` and `sky_decode_kernel` this
-tool finds the innermost loop that holds the most `LEA.HI` (one per MD5 step: `b + rotl(t, s)`), sums its stalls and
-follows each step's dependent chain back from its `LEA.HI` to the previous step's, through the source written last.
+of the stall counts over the loop is the loop's time in cycles.  For `sky_fused_kernel`, `sky_fused_xxh_kernel` and
+`sky_decode_kernel` this tool finds the innermost loop that holds the most `LEA.HI` (one per MD5 step: `b + rotl(t, s)`),
+sums its stalls and follows each step's dependent chain back from its `LEA.HI` to the previous step's, through the source
+written last.
 
     python tools/md5_schedule.py [--lib path/to/libskychunk.so] [--json]
 """
@@ -23,6 +24,7 @@ from pathlib import Path
 LIB = Path(__file__).resolve().parent.parent / "skyplane_b200" / "libskychunk.so"
 KERNELS = {
     "fused": "_ZN3sky16sky_fused_kernelENS_6ParamsE",
+    "fused_xxh": "_ZN3sky20sky_fused_xxh_kernelENS_6ParamsE",  # SKY_F_CHECKSUM: XXH32 stripes between the MD5 rounds
     "decode": "_ZN3sky17sky_decode_kernelENS_9DecParamsE",
 }
 # Execution pipe of the opcodes that can sit on the chain (sm_90: ALU = integer logic/add/shift, FMA = IMAD forms).

@@ -1,7 +1,10 @@
 #!/usr/bin/env python
 """Kernel-only sweeps on one GPU (device-resident inputs): stage flags x workload x chunk size.
 Writes one JSON line per configuration.  Used to fill profiles/ and DESIGN.md tables; not a bench line.
-Flag sets: lz4, md5, both (the fused kernel), hc (SKY_F_HC: high-ratio frames + MD5), hc-lz4 (high-ratio frames only).
+Flag sets: lz4, md5, both (the fused kernel), hc (SKY_F_HC: high-ratio frames + MD5), hc-lz4 (high-ratio frames only),
+checksum / hc-checksum (SKY_F_CHECKSUM: frames with LZ4's content checksum, fast or high-ratio).
+--decode-from liblz4[-linked][-checksums] times the receiver on liblz4's level-0 frames made on the host from the same
+input: independent or linked blocks, without checksums or with block and content checksums.
 --ref-ratio adds the reference's ratio (liblz4 level 0, linked blocks) on the distinct chunks; --liblz4-level9 times liblz4
 level 9 with independent blocks on all of the host's cores (the rate the reference's sender would get from that level)."""
 import argparse
@@ -68,6 +71,28 @@ def liblz4_level9_all_cores(chunks, rounds=2):
     return {"liblz4_level9_indep_cores": n, "liblz4_level9_gbs": raw / dt / 1e9, "liblz4_level9_ratio": raw / sum(sizes)}
 
 
+def liblz4_frames(d_in, stride, n, chunk_bytes, d_out, dst_off, linked, checksums):
+    """liblz4 level-0 frames (linked or independent blocks; with block and content checksums if `checksums`) of the n device chunks,
+    made on the host and copied to d_out at dst_off; the frames of the first 16 distinct chunks are kept for repeats (the
+    Silesia-like input cycles through 8).  -> frame lengths."""
+    import hashlib
+
+    from tools import hc_model
+
+    cache, lens = {}, []
+    for i in range(n):
+        data = d_in[i * stride : i * stride + chunk_bytes].cpu().numpy().tobytes()
+        key = hashlib.sha1(data).digest()
+        f = cache.get(key)
+        if f is None:
+            f = hc_model.liblz4_frame(data, 0, linked, content_checksum=checksums, block_checksum=checksums)
+            if len(cache) < 16:
+                cache[key] = f
+        d_out[dst_off[i] : dst_off[i] + len(f)] = torch.frombuffer(bytearray(f), dtype=torch.uint8).to(d_out.device)
+        lens.append(len(f))
+    return lens
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--total-mib", type=int, default=2048)
@@ -76,12 +101,14 @@ def main():
     ap.add_argument("--flags", default="lz4,md5,both")
     ap.add_argument("--iters", type=int, default=3)
     ap.add_argument("--decode", action="store_true", help="also time the receiver-side decode + MD5 of the frames")
-    ap.add_argument("--decode-from", default="both", help="flag set whose frames --decode times (both, hc)")
+    ap.add_argument("--decode-from", default="both", help="flag set whose frames --decode times (both, hc, checksum, ...), or liblz4[-linked][-checksums] "
+                    "(frames made on the host by liblz4: linked blocks, block and content checksums)")
     ap.add_argument("--ref-ratio", action="store_true", help="also the reference's ratio on the distinct chunks (CPU)")
     ap.add_argument("--liblz4-level9", action="store_true", help="also liblz4 level 9 on all host cores (CPU)")
     a = ap.parse_args()
     dev = torch.device("cuda", 0)
-    FL = {"lz4": native.F_LZ4, "md5": native.F_MD5, "both": 0, "hc": native.F_HC, "hc-lz4": native.F_HC | native.F_LZ4}
+    FL = {"lz4": native.F_LZ4, "md5": native.F_MD5, "both": 0, "hc": native.F_HC, "hc-lz4": native.F_HC | native.F_LZ4,
+          "checksum": native.F_CHECKSUM, "hc-checksum": native.F_HC | native.F_CHECKSUM}
     for wl in a.workloads.split(","):
         for sz in a.sizes_mib.split(","):
             chunk_bytes = int(float(sz) * (1 << 20))
@@ -98,8 +125,8 @@ def main():
                     row.update(liblz4_level9_all_cores(chunks))
                 print(json.dumps(row), flush=True)
             d_in, stride = make_input(wl, n, chunk_bytes, dev)
-            bound = native.frame_bound(chunk_bytes)
-            so = native.round16(bound)
+            bound = native.frame_bound(chunk_bytes) + native.CHECKSUM_BYTES  # (room for a content checksum)
+            so = native.round16(bound + 4 * (chunk_bytes // 65536 + 1))  # (and for liblz4's block checksums, --decode-from)
             d_out = torch.empty(n * so + 64, dtype=torch.uint8, device=dev)
             ctx = native.Context(0, n * stride, n, 0)
             src_off = [i * stride for i in range(n)]
@@ -117,8 +144,14 @@ def main():
                                   "ratio": (tot / sum(out_lens)) if sum(out_lens) else None, "per_stream_gbs": chunk_bytes / k / 1e6}), flush=True)
             if a.decode:
                 # receiver side: decode the frames just produced (d_out) back into a fresh buffer + MD5 of the result
-                out_lens, dg, _ = ctx.process_device(d_in.data_ptr(), src_off, [chunk_bytes] * n, d_out.data_ptr(), dst_off, [bound] * n,
-                                                     FL[a.decode_from], 0)
+                if a.decode_from.startswith("liblz4"):
+                    out_lens = liblz4_frames(d_in, stride, n, chunk_bytes, d_out, dst_off, "-linked" in a.decode_from,
+                                             a.decode_from.endswith("-checksums"))
+                    dg = ctx.process_device(d_in.data_ptr(), src_off, [chunk_bytes] * n, d_out.data_ptr(), dst_off, [bound] * n,
+                                            native.F_MD5, 0)[1]
+                else:
+                    out_lens, dg, _ = ctx.process_device(d_in.data_ptr(), src_off, [chunk_bytes] * n, d_out.data_ptr(), dst_off, [bound] * n,
+                                                         FL[a.decode_from], 0)
                 d_back = torch.empty_like(d_in)
                 ms = []
                 for it in range(a.iters + 1):
