@@ -64,6 +64,13 @@ extern "C" {
  * LZ4 + MD5 + HC, as 0 means LZ4 + MD5; with stage bits it needs SKY_F_LZ4 (SKY_F_MD5 | SKY_F_HC is SKY_E_INVALID).
  * The digests come from the fused kernel's MD5-only mode running beside the HC kernel (two launches per batch). */
 #define SKY_F_HC 32u
+/* high-ratio level (python-lz4's compression_level, liblz4's hash-chain levels): bits 8..11 of flags hold a level
+ * l in 3..9, and the search walks 2^(l-1) chain candidates per position -- more ratio for more GPU time.  A level field
+ * of 0 with SKY_F_HC means level 5 (16 candidates), so SKY_F_HC_LEVEL(5) and SKY_F_HC make the same frames.  A level
+ * field without SKY_F_HC, or outside 3..9, is SKY_E_INVALID.  The frame format does not depend on the level; the level
+ * combines with SKY_F_CHECKSUM, SKY_F_E2EE and the stage bits as SKY_F_HC does.  sky_kernel_config(7) is the highest
+ * level the library supports. */
+#define SKY_F_HC_LEVEL(l) (SKY_F_HC | ((uint32_t)(l) << 8))
 /* content checksum (sky_submit, with or without SKY_F_HC / SKY_F_E2EE, and sky_process_device): the frame carries
  * XXH32(chunk, seed 0) as LZ4's content checksum, so any LZ4 decoder (lz4.frame.decompress, liblz4) verifies that it
  * restores the chunk's bytes.  FLG becomes 0x6C (0x64 for an empty chunk, a 15-byte frame) and the frame ends with the
@@ -84,8 +91,9 @@ SKY_API int sky_device_count(int *count);
 SKY_API int sky_device_pci_bus_id(int device, char *buf, int len);
 /* Compile-time constants of the kernels in this build (tuning builds differ): what = 0 -> LZ4 match-table entries per
  * CTA, 1 -> warps per CTA of the fused kernel, 2 -> probe slots per segment, 3 -> log2 of the largest probe stride;
- * SKY_F_HC: 4 -> chain candidates searched per position, 5 -> log2 of the hash-head entries, 6 -> length at which a
- * position's search stops.  Unknown `what` returns 0 (so a library without SKY_F_HC reads 0 for 4..6).  Parity tests feed
+ * SKY_F_HC: 4 -> chain candidates searched per position at the default level (5), 5 -> log2 of the hash-head entries,
+ * 6 -> length at which a position's search stops, 7 -> highest SKY_F_HC_LEVEL.  Unknown `what` returns 0 (so a library
+ * without SKY_F_HC reads 0 for 4..6, and one without levels 0 for 7).  Parity tests feed
  * these to the sequential twins of the compressors (tools/lz4_tile_model.c, tools/lz4hc_model.c). */
 SKY_API uint32_t sky_kernel_config(int what);
 

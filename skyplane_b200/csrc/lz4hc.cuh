@@ -8,8 +8,9 @@
 //   chains : warp 0 inserts the positions 32 at a time.  A lane's predecessor is the highest lower lane with its hash
 //            (match.any), else head[hash]; then the highest lane of each hash writes head.  That is sequential insertion.
 //            chain[p] is the distance to p's predecessor (u16, 0 = none), head[h] the latest position + 1 (u16, 0 = none);
-//   search : every thread takes positions tid, tid + 1024, ...: walk at most kHcDepth candidates nearest first, keep the
-//            longest common prefix up to min(kHcNice, matchlimit - p), the nearer one on a tie, stop at the cap.  Lengths
+//   search : every thread takes positions tid, tid + 1024, ...: walk at most kHcDepth (the level's depth) candidates
+//            nearest first, keep the longest common prefix up to min(kHcNice, matchlimit - p), the nearer one on a tie,
+//            stop at the cap.  Lengths
 //            (u8) and offsets (u16) go to the CTA's scratch in global memory (L2-resident); the lengths are then copied
 //            back into shared memory over the chains, which the parse no longer needs;
 //   parse  : warp 0 scans 32 positions per step: a position starts a match when its length is >= 4 and the next
@@ -22,10 +23,11 @@
 
 namespace sky {
 
-#ifndef SKY_HC_DEPTH
-#define SKY_HC_DEPTH 16
-#endif
-constexpr uint32_t kHcDepth = SKY_HC_DEPTH;  // chain candidates walked per position
+// Levels (SKY_F_HC_LEVEL): liblz4's hash-chain levels 3..9, defined by the search budget -- level L walks 2^(L-1) chain
+// candidates per position.  Everything else (hash, chains, tie rule, stop length, lazy rule, emission) is the same at every
+// level; the kernel is instantiated once per level, so each depth is a compile-time loop bound.
+constexpr int kHcMinLevel = 3, kHcMaxLevel = 9, kHcDefaultLevel = 5;
+__host__ __device__ constexpr uint32_t hc_depth(int level) { return 1u << (level - 1); }
 constexpr uint32_t kHcHashBits = 14;         // head table: 1 << 14 entries
 constexpr uint32_t kHcNice = 32;             // a position's search stops at this length; the parse extends such matches
 constexpr int kHcWarps = 32;
@@ -48,6 +50,7 @@ static_assert(kHcSmemBytes <= 232448, "one HC CTA per SM: at most 227 KiB of sha
 constexpr uint32_t kHcLenOff = 0, kHcOffOff = kBlock, kHcOutOff = 3 * kBlock;
 constexpr uint32_t kHcScratchBytes = 4 * kBlock + 2048;
 
+template <uint32_t kHcDepth>  // chain candidates walked per position: hc_depth(level)
 __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;

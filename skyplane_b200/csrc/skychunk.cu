@@ -591,6 +591,19 @@ struct HcArrays {  // SKY_F_HC: the HC kernel's scratch, and the stream the dige
     Stream md5_stream;
     Event ev_fork, ev_join;
 };
+// the HC kernel of each level, kHcMinLevel .. kHcMaxLevel
+using HcKernel = void (*)(const Params);
+static const HcKernel kHcKernels[] = {sky_hc_kernel<hc_depth(3)>, sky_hc_kernel<hc_depth(4)>, sky_hc_kernel<hc_depth(5)>,
+                                      sky_hc_kernel<hc_depth(6)>, sky_hc_kernel<hc_depth(7)>, sky_hc_kernel<hc_depth(8)>,
+                                      sky_hc_kernel<hc_depth(9)>};
+static_assert(sizeof(kHcKernels) / sizeof(kHcKernels[0]) == kHcMaxLevel - kHcMinLevel + 1, "one HC kernel per level");
+constexpr uint32_t kHcLevelShift = 8, kHcLevelMask = 0xfu << kHcLevelShift;  // SKY_F_HC_LEVEL's field in `flags`
+static_assert(SKY_F_HC_LEVEL(1) == (SKY_F_HC | (1u << kHcLevelShift)), "the level field of include/skychunk.h");
+// The level a batch's flags select: the level field, or kHcDefaultLevel when it is 0.
+static int hc_level(uint32_t flags) {
+    const int l = (int)((flags & kHcLevelMask) >> kHcLevelShift);
+    return l ? l : kHcDefaultLevel;
+}
 struct DecodeArrays {  // receiver side
     PinnedMem<DecChunk> h_chunks; DevMem<DecChunk> d_chunks;
     PinnedMem<int32_t> h_status; DevMem<int32_t> d_status;
@@ -801,9 +814,10 @@ uint32_t sky_kernel_config(int what) {
     case 1: return (uint32_t)kWarps;
     case 2: return kSegSlots;
     case 3: return kMaxStepLog;
-    case 4: return kHcDepth;
+    case 4: return hc_depth(kHcDefaultLevel);
     case 5: return kHcHashBits;
     case 6: return kHcNice;
+    case 7: return (uint32_t)kHcMaxLevel;
     default: return 0;
     }
 }
@@ -835,7 +849,8 @@ int sky_ctx_create(int device, uint64_t max_batch_bytes, uint32_t max_chunks, ui
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_xxh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_xxh_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_hc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
+    for (const HcKernel k : kHcKernels)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
     if (e != cudaSuccess) {
         g_err = ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (this build carries sm_90a code only)";
         return SKY_E_CUDA;
@@ -951,8 +966,10 @@ static uint32_t fill_md5_order(uint32_t *order, uint32_t n, const uint64_t *len)
 }
 
 // SKY_F_HC selects how frames are made and SKY_F_CHECKSUM adds to the frame, so each needs SKY_F_LZ4, or no stage bit at
-// all (= LZ4 + MD5).
+// all (= LZ4 + MD5).  A level field needs SKY_F_HC and a level in kHcMinLevel .. kHcMaxLevel.
 static bool frame_flags_valid(uint32_t flags) {
+    if ((flags & kHcLevelMask) && (!(flags & SKY_F_HC) || hc_level(flags) < kHcMinLevel || hc_level(flags) > kHcMaxLevel))
+        return false;
     return !(flags & (SKY_F_HC | SKY_F_CHECKSUM)) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5;
 }
 // Bytes a chunk's frame may take: SKY_F_CHECKSUM adds the 4-byte content checksum behind the EndMark.
@@ -1027,7 +1044,7 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
             ctx->launches++;
         }
         p.scratch = h.scratch;
-        sky_hc_kernel<<<ctx->sm_count, kHcThreads, kHcSmemBytes, st>>>(p);
+        kHcKernels[hc_level(flags) - kHcMinLevel]<<<ctx->sm_count, kHcThreads, kHcSmemBytes, st>>>(p);
         CK(ctx, cudaGetLastError());
         if (md5) CK(ctx, cudaStreamWaitEvent(st, h.ev_join, 0));
     } else {

@@ -57,12 +57,13 @@ def run_stream(
     n_slots: int = 4,
     high_ratio: bool = False,
     content_checksum: bool = False,
+    compression_level: Optional[int] = None,
 ) -> Dict:
     """Stream ``n_requests`` chunk requests (recycling ``pool_files`` by hard link) through the operator.
 
     The first ``warmup_requests`` completions are not timed (worker start-up: CUDA context, pinned staging).
-    ``high_ratio`` and ``content_checksum`` are handed to the operator (GatewayCompressHash's high-ratio frames, frames with
-    LZ4's content checksum) when set.
+    ``high_ratio``, ``content_checksum`` and ``compression_level`` are handed to the operator (GatewayCompressHash's
+    high-ratio frames, frames with LZ4's content checksum, the high-ratio level) when set.
     Returns {"wall_s", "bytes", "records": [{chunk_id, pool_index, md5, raw_len, frame_path}], "status": {...}}.
     """
     chunk_dir = Path(chunk_dir)
@@ -75,6 +76,7 @@ def run_stream(
         max_batch_chunks=max_batch_chunks, max_batch_bytes=max_batch_bytes, n_gpus=n_gpus, keep_frames_on_disk=keep_frames, n_slots=n_slots,
         **({"high_ratio": True} if high_ratio else {}),
         **({"content_checksum": True} if content_checksum else {}),
+        **({"compression_level": compression_level} if compression_level is not None else {}),
     )
     op.start_workers()
     records: List[Dict] = []

@@ -16,6 +16,11 @@ SKY_OK = 0
 SKY_E_INVALID, SKY_E_NOGPU, SKY_E_CUDA, SKY_E_CAPACITY, SKY_E_BUSY, SKY_E_TICKET, SKY_E_NOMEM, SKY_E_NOKEY = -1, -2, -3, -4, -5, -6, -7, -8
 F_LZ4, F_MD5, F_E2EE, F_HC, F_CHECKSUM = 1, 2, 16, 32, 64
 CHECKSUM_BYTES = 4  # F_CHECKSUM: the content checksum (u32le XXH32) behind the EndMark
+# SKY_F_HC_LEVEL(l): the high-ratio level l (3..9: 2**(l - 1) chain candidates per position) in bits 8..11 of the flags;
+# a level field of 0 with F_HC is the default level
+HC_LEVEL_SHIFT = 8
+HC_LEVEL_MASK = 0xF << HC_LEVEL_SHIFT
+HC_MIN_LEVEL, HC_DEFAULT_LEVEL, HC_MAX_LEVEL = 3, 5, 9
 BOX_OVERHEAD = 40
 # sky_decode status codes
 D_OK, D_BAD_HEADER, D_CORRUPT, D_SIZE, D_UNSUPPORTED, D_LAYOUT, D_TRUNCATED, D_AUTH, D_CHECKSUM = 0, -1, -2, -3, -4, -5, -6, -7, -8
@@ -129,11 +134,44 @@ def device_pci_bus_id(device: int) -> str:
 
 
 def kernel_config() -> dict:
-    """Compile-time constants of the loaded build (sky_kernel_config); the hc_* keys read 0 on a library without F_HC."""
+    """Compile-time constants of the loaded build (sky_kernel_config); the hc_* keys read 0 on a library without F_HC
+    (hc_depth is the default level's; hc_max_level reads 0 on a library without levels)."""
     L = lib()
     return {"lz4_entries": L.sky_kernel_config(0), "warps": L.sky_kernel_config(1), "seg_slots": L.sky_kernel_config(2),
             "max_step_log": L.sky_kernel_config(3), "hc_depth": L.sky_kernel_config(4), "hc_hash_bits": L.sky_kernel_config(5),
-            "hc_nice": L.sky_kernel_config(6)}
+            "hc_nice": L.sky_kernel_config(6), "hc_max_level": L.sky_kernel_config(7)}
+
+
+def hc_depth(level: int) -> int:
+    """Chain candidates the high-ratio search walks per position at `level` (liblz4's hash-chain levels)."""
+    return 1 << (level - 1)
+
+
+def hc_level_flag(level: int) -> int:
+    """SKY_F_HC_LEVEL(level): the flags of the high-ratio mode at `level` (3..9)."""
+    if isinstance(level, bool) or not isinstance(level, int) or not HC_MIN_LEVEL <= level <= HC_MAX_LEVEL:
+        raise ValueError(f"high-ratio levels are {HC_MIN_LEVEL}..{HC_MAX_LEVEL}, not {level!r}")
+    return F_HC | (level << HC_LEVEL_SHIFT)
+
+
+def hc_flags(level: Optional[int] = None, hc: bool = False, compress: bool = True) -> int:
+    """python-lz4's ``compression_level`` (and the stage's ``hc`` switch) -> the flag bits that choose the compressor:
+    0 (the fast path), F_HC (hc=True without a level: the default level 5) or hc_level_flag(level).  Levels 3..9 select the
+    high-ratio mode at that level; 0..2 are the fast compressor, so they contradict hc=True.  A level with compress=False,
+    or outside 0..9, is a ValueError (10..12 are liblz4's optimal parser, which the stage does not have)."""
+    if level is None:
+        return F_HC if hc else 0
+    if isinstance(level, bool) or not isinstance(level, int):
+        raise ValueError(f"compression_level must be an int, not {level!r}")
+    if not compress:
+        raise ValueError("compression_level selects how frames are compressed: it needs compression")
+    if not 0 <= level <= HC_MAX_LEVEL:
+        raise ValueError(f"compression_level {level} is not supported: 0..2 (fast) or {HC_MIN_LEVEL}..{HC_MAX_LEVEL} (high-ratio)")
+    if level < HC_MIN_LEVEL:
+        if hc:
+            raise ValueError(f"compression_level {level} is the fast compressor: the high-ratio mode takes {HC_MIN_LEVEL}..{HC_MAX_LEVEL}")
+        return 0
+    return hc_level_flag(level)
 
 
 def frame_bound(n: int) -> int:

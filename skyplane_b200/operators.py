@@ -135,6 +135,7 @@ class GatewayCompressHash(GatewayOperator):
         n_slots: int = 4,
         high_ratio: bool = False,
         content_checksum: bool = False,
+        compression_level: Optional[int] = None,
     ):
         """use_compression / e2ee_key_bytes: GatewaySender's arguments of the same name (gateway_operator.py:154-168):
         ``use_compression=False`` digests the chunk and lets it pass through uncompressed (``is_compressed=False``);
@@ -144,6 +145,9 @@ class GatewayCompressHash(GatewayOperator):
         content_checksum: every frame carries LZ4's content checksum (XXH32 of the chunk, python-lz4's argument of the same
         name), so any receiver that decodes it with ``lz4.frame.decompress`` verifies the chunk's bytes end to end; the GPU
         receiver verifies it too.  Needs ``use_compression``.
+        compression_level: python-lz4's argument of the same name (``ChunkStage.launch(level=...)``): 3..9 makes the
+        frames with the high-ratio parse at that level (2**(level - 1) chain candidates per position, more ratio for more GPU
+        time), 0..2 with the fast compressor; ``high_ratio`` alone means level 5.  Needs ``use_compression``.
         sink: ``callable(worker_id) -> socket``, called once in each worker.  With a sink the worker sends every payload
         straight from the pinned staging slot (``wire.send_results``: WireProtocolHeader + payload, no intermediate bytes
         object, no frame file) -- the tail of ``GatewaySender.process`` (gateway_operator.py:367-402)."""
@@ -155,6 +159,10 @@ class GatewayCompressHash(GatewayOperator):
         if content_checksum and not self.use_compression:
             raise ValueError("content_checksum is carried by the LZ4 frame: it needs use_compression")
         self.content_checksum = bool(content_checksum)
+        from skyplane_b200 import native
+
+        native.hc_flags(compression_level, self.high_ratio, self.use_compression)  # (ValueError on a bad level, here and not in a worker)
+        self.compression_level = compression_level
         self.e2ee_key_bytes = e2ee_key_bytes
         self.sink = sink
         # batches in flight per worker: a batch of 8 MiB chunks spends >= 70 ms on the GPU whatever its size (one serial MD5
@@ -300,6 +308,8 @@ class GatewayCompressHash(GatewayOperator):
         opts = {"hc": True} if self.high_ratio else {}
         if self.content_checksum:
             opts["checksum"] = True
+        if self.compression_level is not None:
+            opts["level"] = self.compression_level
         stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None, **opts)
         return True
 

@@ -33,6 +33,7 @@ def _compress_hash(op: Dict, kw: Dict) -> GatewayOperator:
         use_compression=op.get("compress", True),
         high_ratio=op.get("high_ratio", False),
         content_checksum=op.get("content_checksum", False),
+        compression_level=op.get("compression_level"),
         max_batch_chunks=op.get("max_batch_chunks", 64),
         max_batch_bytes=op.get("max_batch_bytes", 512 << 20),
         n_gpus=op.get("num_gpus"),

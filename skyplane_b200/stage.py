@@ -157,22 +157,27 @@ class ChunkStage:
         self._has_key = key is not None
 
     def launch(self, slot: _Slot, compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None, hc: bool = False,
-               checksum: bool = False) -> _Slot:
+               checksum: bool = False, level: Optional[int] = None) -> _Slot:
         """compress=False is the reference's `compress: false` (digest only, the chunk passes through);
         encrypt=True seals every payload with the stage's key (nonces: 24 bytes per chunk, default os.urandom);
         hc=True makes the frames with the high-ratio parse (F_HC): same frame format, fewer bytes, more GPU time;
-        checksum=True gives every frame LZ4's content checksum (F_CHECKSUM), which any LZ4 decoder verifies."""
+        checksum=True gives every frame LZ4's content checksum (F_CHECKSUM), which any LZ4 decoder verifies;
+        level is python-lz4's compression_level: 3..9 runs the high-ratio parse at that level (2**(level - 1) chain
+        candidates per position: more ratio for more GPU time), hc=True alone means level 5, 0..2 is the fast path."""
         if not slot.lens:
             raise ValueError("empty batch")
         if hc and not compress:
             raise ValueError("hc=True selects how frames are compressed: it needs compress=True")
         if checksum and not compress:
             raise ValueError("checksum=True is carried by the LZ4 frame: it needs compress=True")
-        if hc and not native.kernel_config()["hc_depth"]:
+        hc_bits = native.hc_flags(level, hc, compress)
+        if hc_bits and not native.kernel_config()["hc_depth"]:
             raise native.SkyChunkError(native.SKY_E_INVALID, f"{native.LIB_PATH.name} was built without the high-ratio kernel (F_HC)")
+        if hc_bits & native.HC_LEVEL_MASK and native.kernel_config()["hc_max_level"] < level:
+            raise native.SkyChunkError(native.SKY_E_INVALID, f"{native.LIB_PATH.name} was built without high-ratio level {level}")
         base_in, base_out = slot.inp.addr, slot.out.addr
         src = [base_in + o for o in slot.in_off]
-        flags = (native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0) | (native.F_HC if hc else 0)
+        flags = (native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0) | hc_bits
                  | (native.F_CHECKSUM if checksum else 0))
         if encrypt and nonces is None:
             nonces = os.urandom(24 * len(slot.lens))  # what nacl.utils.random(24) draws per message
@@ -199,9 +204,10 @@ class ChunkStage:
 
     # ------------------------------------------------------------------ sync convenience
     def process(self, chunks: Sequence[BytesLike], compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None,
-                hc: bool = False, checksum: bool = False) -> List[StageResult]:
-        """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes (hc, checksum:
-        see launch)."""
+                hc: bool = False, checksum: bool = False, level: Optional[int] = None) -> List[StageResult]:
+        """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes (hc, checksum,
+        level: see launch)."""
+        native.hc_flags(level, hc, compress)  # (bad arguments fail before the first batch)
         out: List[StageResult] = []
         i = 0
         while i < len(chunks):
@@ -213,7 +219,7 @@ class ChunkStage:
             if j == i:
                 self.release(slot)
                 raise native.SkyChunkError(native.SKY_E_CAPACITY, f"chunk of {memoryview(chunks[i]).nbytes} bytes exceeds max_batch_bytes")
-            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum)
+            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum, level)
             for r in self.collect(slot):
                 out.append(StageResult(frame=memoryview(bytes(r.frame)), md5=r.md5, raw_len=r.raw_len, comp_len=r.comp_len,
                                        is_compressed=r.is_compressed, is_encrypted=r.is_encrypted))

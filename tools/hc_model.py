@@ -18,8 +18,13 @@ class Opts(ctypes.Structure):
     _fields_ = [("depth", ctypes.c_int), ("hash_bits", ctypes.c_int), ("nice", ctypes.c_int)]
 
 
-def kernel_opts(depth: int = 16, hash_bits: int = 14, nice: int = 32) -> Opts:
-    """The constants skyplane_b200/csrc/lz4hc.cuh is built with (sky_kernel_config(4), (5), (6))."""
+def kernel_opts(depth: int = 16, hash_bits: int = 14, nice: int = 32, level: int | None = None) -> Opts:
+    """The constants skyplane_b200/csrc/lz4hc.cuh is built with (sky_kernel_config(4), (5), (6)); `level` (3..9,
+    SKY_F_HC_LEVEL) replaces the default level's depth with that level's, 2**(level - 1)."""
+    if level is not None:
+        if not 3 <= level <= 9:
+            raise ValueError(f"high-ratio levels are 3..9, not {level}")
+        depth = 1 << (level - 1)
     return Opts(depth, hash_bits, nice)
 
 

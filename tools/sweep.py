@@ -2,7 +2,8 @@
 """Kernel-only sweeps on one GPU (device-resident inputs): stage flags x workload x chunk size.
 Writes one JSON line per configuration.  Used to fill profiles/ and DESIGN.md tables; not a bench line.
 Flag sets: lz4, md5, both (the fused kernel), hc (SKY_F_HC: high-ratio frames + MD5), hc-lz4 (high-ratio frames only),
-checksum / hc-checksum (SKY_F_CHECKSUM: frames with LZ4's content checksum, fast or high-ratio).
+checksum / hc-checksum (SKY_F_CHECKSUM: frames with LZ4's content checksum, fast or high-ratio), hc3 .. hc9 and
+hc3-checksum .. hc9-checksum (SKY_F_HC_LEVEL(3..9): the high-ratio mode at that level; hc5 makes hc's frames).
 --decode-from liblz4[-linked][-checksums] times the receiver on liblz4's level-0 frames made on the host from the same
 input: independent or linked blocks, without checksums or with block and content checksums.
 --ref-ratio adds the reference's ratio (liblz4 level 0, linked blocks) on the distinct chunks; --liblz4-level9 times liblz4
@@ -109,6 +110,9 @@ def main():
     dev = torch.device("cuda", 0)
     FL = {"lz4": native.F_LZ4, "md5": native.F_MD5, "both": 0, "hc": native.F_HC, "hc-lz4": native.F_HC | native.F_LZ4,
           "checksum": native.F_CHECKSUM, "hc-checksum": native.F_HC | native.F_CHECKSUM}
+    for lv in range(native.HC_MIN_LEVEL, native.HC_MAX_LEVEL + 1):
+        FL[f"hc{lv}"] = native.hc_level_flag(lv)
+        FL[f"hc{lv}-checksum"] = native.hc_level_flag(lv) | native.F_CHECKSUM
     for wl in a.workloads.split(","):
         for sz in a.sizes_mib.split(","):
             chunk_bytes = int(float(sz) * (1 << 20))
