@@ -30,6 +30,12 @@ constexpr int32_t kDecLayout = -5;      // block structure does not match 64 KiB
 constexpr int32_t kDecTruncated = -6;   // frame ends inside a header, block, checksum or before the content checksum
 constexpr int32_t kDecChecksum = -8;    // a block checksum or the content checksum does not match (-7 is SKY_D_AUTH)
 
+// While blocks decode, a chunk's status may hold block_fail(j, code): below every code above, and ordered by block index
+// first, so atomicMin keeps the earliest failing block.  Once every block is done, the chunk's MD5 lane turns it back
+// into `code`.
+constexpr int32_t kBlockFail = INT32_MIN;
+__device__ __forceinline__ int32_t block_fail(uint32_t j, int32_t code) { return kBlockFail + (int32_t)(j * 16u) - code; }
+
 constexpr uint32_t kChkBlock = 1, kChkContent = 2;  // DecChunk::checks
 
 struct DecChunk {

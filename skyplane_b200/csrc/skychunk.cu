@@ -403,7 +403,7 @@ struct DecParams {
     uint32_t *counter;   // work counter
     uint32_t *blk_done;  // per block: 1 once decoded (gates the MD5 lanes)
     const uint32_t *md5_order;
-    uint8_t *md5_out;    // null = no digest
+    uint8_t *md5_out;    // 16 bytes per chunk (every chunk has an MD5 lane, which also settles its status)
     uint32_t n_chunks;
     uint32_t n_groups;
     uint32_t rows;
@@ -445,7 +445,7 @@ struct DecRowGate {
 __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (p.md5_out && warp < kMd5WarpsPerCta) {
+    if (warp < kMd5WarpsPerCta) {
         const uint32_t md5_slots = gridDim.x * kMd5WarpsPerCta;
         for (uint32_t g = warp * gridDim.x + blockIdx.x; g < p.n_groups; g += md5_slots) {
             const uint32_t c = p.md5_order[g * 32 + lane];
@@ -460,11 +460,19 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
             }
             const uint32_t x = md5_warp<true>(reinterpret_cast<uint32_t *>(smem + warp * kRingBytes), src, len, active,
                                               p.md5_out + (size_t)(active ? c : 0) * 16, lane, gate);
-            // every row has passed the gate, so the chunk's decode status is final: a checksum mismatch only replaces ok
-            if (active && (p.chunks[c].checks & kChkContent) && x != p.chunks[c].content_xxh) atomicCAS(p.status + c, kDecOk, kDecChecksum);
+            // every row has passed the gate, so no decode warp writes the status any more: settle a block failure into its
+            // code (lz4dec.cuh, block_fail); a content checksum mismatch only replaces ok
+            if (active) {
+                const int32_t s = *reinterpret_cast<volatile int32_t *>(p.status + c);
+                if (s < kDecChecksum) p.status[c] = -((s - kBlockFail) & 15);
+                else if ((p.chunks[c].checks & kChkContent) && x != p.chunks[c].content_xxh) atomicCAS(p.status + c, kDecOk, kDecChecksum);
+            }
             __syncwarp();
         }
     }
+    // A failing block folds block_fail(j, code) into the chunk's status with atomicMin, so the earliest failing block wins
+    // whichever warp gets there first (liblz4 checks and decodes blocks in order and reports the first error); the chunk's
+    // MD5 lane turns it back into that block's code.  A block is skipped only once the header or an earlier block failed.
     const uint32_t total = p.rows * p.n_chunks;
     for (;;) {
         uint32_t w = 0;
@@ -488,18 +496,18 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
             __syncwarp();
             st = *reinterpret_cast<volatile int32_t *>(p.status + c);
         }
-        if (st == kDecOk) {
+        if (st == kDecOk || (st < kDecChecksum && st > block_fail(j, 0))) {  // no failure yet, or only in later blocks
             const DecBlock b = p.blocks[cd.blk_base + j];
             const uint32_t sz = b.word & 0x7FFFFFFFu;
             if ((cd.checks & kChkBlock) && xxh32_warp(cd.frame + b.off, sz, lane) != b.chk) {
                 st = kDecChecksum;
             } else if (b.word & 0x80000000u) {
-                if (sz != want) st = kDecLayout;
-                else warp_copy(cd.out + pos, cd.frame + b.off, sz, lane);
+                st = sz != want ? kDecLayout : kDecOk;
+                if (st == kDecOk) warp_copy(cd.out + pos, cd.frame + b.off, sz, lane);
             } else {
                 st = lz4_decode_block(cd.frame + b.off, sz, cd.out, pos, want, cd.linked ? 0 : pos, lane);
             }
-            if (st != kDecOk && lane == 0) atomicMin(p.status + c, st);
+            if (st != kDecOk && lane == 0) atomicMin(p.status + c, block_fail(j, st));
         }
         __syncwarp();
         if (lane == 0) {
