@@ -18,7 +18,8 @@
  * restores bit-exactly: magic, FLG=0x68 (v01, independent blocks, content size), BD=0x40 (64 KiB),
  * u64le content size, header checksum, blocks (bit 31 set = stored raw), EndMark.  A zero-length
  * chunk yields the 11-byte frame liblz4 itself emits (content size omitted).  With SKY_F_CHECKSUM the
- * frame also carries LZ4's content checksum (FLG=0x6C, u32le XXH32 of the chunk after the EndMark).
+ * frame also carries LZ4's content checksum (FLG=0x6C, u32le XXH32 of the chunk after the EndMark), with
+ * SKY_F_BLOCK_CHECKSUM a block checksum behind every block (FLG=0x78).
  * The receiver accepts block and content checksums in any frame and verifies them (SKY_D_CHECKSUM).
  */
 #ifndef SKYCHUNK_H
@@ -79,6 +80,16 @@ extern "C" {
  * XXH32, so the digests always come back; without SKY_F_LZ4 (no frame to carry it) it is SKY_E_INVALID.  One more launch
  * per batch writes the checksums into the frames. */
 #define SKY_F_CHECKSUM 64u
+/* block checksums (sky_submit, with or without SKY_F_HC / SKY_F_HC_LEVEL, SKY_F_CHECKSUM and SKY_F_E2EE, and
+ * sky_process_device): every block's data is followed by u32le XXH32(block data as stored in the frame, seed 0) -- the
+ * compressed bytes, or the raw bytes of a stored block -- as liblz4 writes with blockChecksumFlag = 1, so any LZ4 decoder
+ * (lz4.frame.decompress, liblz4, sky_decode) rejects a damaged block by its own checksum before decoding it.  FLG becomes
+ * 0x78 (0x7C with SKY_F_CHECKSUM; 0x70 / 0x74 for an empty chunk, which has no block); the EndMark, the content checksum
+ * and out_len move by 4 bytes per block, and dst_cap[i] >= sky_frame_bound(src_len[i]) + 4 * ceil(src_len[i] / 65536)
+ * (+ 4 with SKY_F_CHECKSUM, + SKY_BOX_OVERHEAD with SKY_F_E2EE).  Alone it means LZ4 + MD5 + block checksums; without
+ * SKY_F_LZ4 (no frame to carry them) it is SKY_E_INVALID.  The compressor CTA that writes a block hashes it; one more
+ * launch per batch writes FLG and the header checksum byte. */
+#define SKY_F_BLOCK_CHECKSUM 128u
 
 typedef struct sky_ctx sky_ctx;
 

@@ -8,6 +8,7 @@
 // on lower-numbered work items, all of which were claimed earlier by running CTAs.
 #pragma once
 #include "lz4.cuh"
+#include "xxh32.cuh"
 
 namespace sky {
 
@@ -116,6 +117,9 @@ struct BlockPlace {
 };
 // One thread, once the block's compressed size is known: wait for the block's frame offset on the OFF chain, hand block
 // j+1 its offset at once, write the block header and, on the chunk's last block, the EndMark and the frame length.
+// kBlkChk (SKY_F_BLOCK_CHECKSUM): 4 more bytes follow the block's data for its checksum (block_checksum writes them), so
+// the next offset is known before any hashing.
+template <bool kBlkChk = false>
 __device__ __forceinline__ BlockPlace place_block(const Params &p, const BlockDesc &d, uint32_t csize, uint32_t L) {
     const bool raw = csize > L - 1;  // LZ4F_makeBlock: a block that does not shrink is stored
     uint64_t *cw = p.chain + d.c;
@@ -126,7 +130,7 @@ __device__ __forceinline__ BlockPlace place_block(const Params &p, const BlockDe
         if (ns < 2048) ns <<= 1;
     }
     const uint64_t off = st & kOffMask;
-    const uint64_t end = off + 4 + (raw ? L : csize);
+    const uint64_t end = off + 4 + (raw ? L : csize) + (kBlkChk ? 4 : 0);
     if (!d.last) st_release(cw, ((uint64_t)(d.j + 1) << kOffBits) | end);
     uint8_t *hdr = d.dst + off;
     const uint32_t hword = raw ? (L | 0x80000000u) : csize;
@@ -146,6 +150,38 @@ __device__ __forceinline__ void copy_block(uint8_t *out, const uint8_t *src, uin
     const uint32_t per = (((n + kNumWarps - 1) / kNumWarps) + 15u) & ~15u;
     const uint32_t lo = warp * per;
     if (lo < n) warp_copy_stream<kReadOnly>(out + lo, src + lo, min(per, n - lo), lane);
+}
+
+// SKY_F_BLOCK_CHECKSUM, one warp: the block checksum -- XXH32 (seed 0) of the block's n data bytes as stored in the frame:
+// the compressed bytes, or the raw bytes of a stored block -- read from `src` and written as u32le at `at`, right behind
+// the data.  place_block<true> has passed the next offset on before any of this, so the hash is never on the OFF chain.
+__device__ __forceinline__ void block_checksum(const uint8_t *src, uint32_t n, uint8_t *at, unsigned lane) {
+    const uint32_t x = xxh32_warp(src, n, lane);
+    if (lane == 0) { at[0] = (uint8_t)x; at[1] = (uint8_t)(x >> 8); at[2] = (uint8_t)(x >> 16); at[3] = (uint8_t)(x >> 24); }
+}
+// A block whose checksum is hashed later from its bytes in the frame, by one warp of the CTA that wrote them, after a CTA
+// barrier has ordered those writes before its reads: the warp runs it where it would otherwise wait, off the CTA's next
+// block (sky_fused_kernel and sky_hc_kernel say where).  It lives in shared memory (a register copy would stay live across
+// the whole block loop), and only the hashing warp reads or writes it once the kernel has cleared it.
+struct PendingChecksum {
+    uint8_t *data;  // the block's first data byte in the frame; null: nothing pending
+    uint32_t n;
+};
+// The hashing warp: hash the pending block, if there is one, and clear it.
+__device__ __forceinline__ void run_pending(PendingChecksum *pc, unsigned lane) {
+    uint8_t *const d = pc->data;
+    const uint32_t n = pc->n;
+    if (!d) return;
+    __syncwarp();  // every lane has read it
+    if (lane == 0) pc->data = nullptr;
+    block_checksum(d, n, d + n, lane);
+}
+__device__ __forceinline__ void set_pending(PendingChecksum *pc, uint8_t *data, uint32_t n, unsigned lane) {
+    __syncwarp();
+    if (lane == 0) {
+        pc->data = data;
+        pc->n = n;
+    }
 }
 
 }  // namespace sky

@@ -39,6 +39,7 @@ struct HcCtl {
     BlockDesc desc;
     uint64_t data;  // frame offset of the block's first data byte
     uint32_t csize, raw;
+    PendingChecksum pend;  // kBlkChk: the CTA's last block until warp 1 hashes it
 };
 constexpr uint32_t kHcInOff = 0;                                  // the block (+ slack for unaligned 4-byte reads)
 constexpr uint32_t kHcChainOff = kInBytes;                        // u16 per position; after the search: u8 length per position
@@ -50,8 +51,11 @@ static_assert(kHcSmemBytes <= 232448, "one HC CTA per SM: at most 227 KiB of sha
 constexpr uint32_t kHcLenOff = 0, kHcOffOff = kBlock, kHcOutOff = 3 * kBlock;
 constexpr uint32_t kHcScratchBytes = 4 * kBlock + 2048;
 
-template <uint32_t kHcDepth>  // chain candidates walked per position: hc_depth(level)
-__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
+// kHcDepth: chain candidates walked per position, hc_depth(level).  kBlkChk (SKY_F_BLOCK_CHECKSUM): every block gets its
+// checksum (block_checksum), hashed from the frame by warp 1 during the next block's chain step, which only warp 0 works
+// on (or before the CTA exits).
+template <uint32_t kHcDepth, bool kBlkChk>
+__device__ __forceinline__ void hc_body(const Params &p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     uint8_t *in = smem + kHcInOff;
@@ -63,6 +67,7 @@ __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
     uint8_t *cout = scr + kHcOutOff;
     if (tid == 0) {
         mbar_init(&ctl->in_full, 1);
+        if constexpr (kBlkChk) ctl->pend.data = nullptr;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -71,7 +76,12 @@ __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
         if (tid == 0) claim_block(p, &ctl->desc);
         __syncthreads();  // (also: every warp is done with the previous block)
         const BlockDesc d = ctl->desc;
-        if (!d.valid) break;
+        if (!d.valid) {
+            if constexpr (kBlkChk) {
+                if (warp == 1) run_pending(&ctl->pend, lane);
+            }
+            break;
+        }
         const uint32_t L = d.L;
         if (tid == 0) load_block(in, d.src, L, &ctl->in_full);
         uint4 *h4 = reinterpret_cast<uint4 *>(smem + kHcHeadOff);
@@ -97,6 +107,9 @@ __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
                 }
                 __syncwarp();
             }
+        }
+        if constexpr (kBlkChk) {
+            if (warp == 1) run_pending(&ctl->pend, lane);  // the previous block's checksum, beside warp 0's chains
         }
         __syncthreads();
         // ---------------------------------------------------------------- best match per position (all warps)
@@ -174,7 +187,7 @@ __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
             }
             op = emit_seq(cout, op, in, anchor, L - anchor, 0, 0, lane);  // the final literals
             if (lane == 0) {
-                const BlockPlace pl = place_block(p, d, op, L);
+                const BlockPlace pl = place_block<kBlkChk>(p, d, op, L);
                 ctl->data = pl.data;
                 ctl->csize = op;
                 ctl->raw = pl.raw;
@@ -185,7 +198,16 @@ __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
         uint8_t *out = d.dst + ctl->data;
         if (ctl->raw) copy_block<kHcWarps, true>(out, d.src, L, warp, lane);
         else copy_block<kHcWarps, false>(out, cout, ctl->csize, warp, lane);
+        if constexpr (kBlkChk) {
+            if (warp == 1) set_pending(&ctl->pend, out, ctl->raw ? L : ctl->csize, lane);
+        }
     }
 }
+
+template <uint32_t kHcDepth>
+__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) { hc_body<kHcDepth, false>(p); }
+// SKY_F_BLOCK_CHECKSUM: the same kernel with block checksums.
+template <uint32_t kHcDepth>
+__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_bc_kernel(const Params p) { hc_body<kHcDepth, true>(p); }
 
 }  // namespace sky

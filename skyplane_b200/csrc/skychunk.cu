@@ -72,6 +72,8 @@ struct Ctl {
     volatile uint32_t seg_hit[4];     // per segment (mod 4): OR of its batches' hit masks (decides the stride two segments on)
     uint32_t raw, last_lits, tail_off;  // plan results: stored?, final literal run and where it goes
     uint64_t data;                      // frame offset of the block's first data byte
+    uint32_t size;                      // the block's data bytes in the frame (kBlkChk only)
+    PendingChecksum pend;               // kBlkChk: the CTA's last compressed block until kSumWarp hashes it
 };
 constexpr uint32_t kInOff = 0;
 constexpr uint32_t kTabOff = kInOff + kInBytes;
@@ -96,7 +98,12 @@ __device__ __forceinline__ void bar_wait() { asm volatile("bar.sync %0, 64;" ::"
 //       when the groups are done the CTA joins the compressors.  kXxh: the MD5 lanes also write XXH32(chunk) to xxh_out.
 //   compressor CTAs: one 64 KiB block at a time -- bulk-load it into shared memory, warp 0 probes, warps 1.. parse
 //       (lz4.cuh), warp 0 plans the block's layout and takes its frame offset from the OFF chain, all warps write it out.
-template <bool kXxh>
+//       kBlkChk (SKY_F_BLOCK_CHECKSUM): the last parser warp also hashes every block the CTA writes (block_checksum).  A
+//       block is only whole in the frame once every warp has written its part, so its hash is deferred to the CTA's next
+//       block: the warp reads it back from the frame between two of its segment claims, and the other parsers take up
+//       its share of the segments meanwhile.  (Hashing a stored block from the block buffer during its own write-out
+//       instead made ptxas spill in the main loop.)
+template <bool kXxh, bool kBlkChk>
 __device__ __forceinline__ void fused_body(const Params &p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -117,6 +124,7 @@ __device__ __forceinline__ void fused_body(const Params &p) {
             mbar_init(&ctl->empty[i], 1);
         }
         ctl->claim = 0;
+        if constexpr (kBlkChk) ctl->pend.data = nullptr;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -151,6 +159,7 @@ __device__ __forceinline__ void fused_body(const Params &p) {
     uint32_t my_seq = 0;      // parser: the sequence number it holds a claim on
     bool have_claim = false;
     uint32_t in_phase = 0;
+    constexpr unsigned kSumWarp = kWarps - 1;  // kBlkChk: the warp that hashes the blocks
     for (uint32_t it = 0;; it++) {
         BlockDesc *dsc = &ctl->desc[it & 1];
         if (warp == 0 && lane == 0) {
@@ -159,7 +168,12 @@ __device__ __forceinline__ void fused_body(const Params &p) {
             ctl->nseg = 0;
         }
         __syncthreads();  // (also: every warp is done with the previous block's buffer, records and plan)
-        if (!dsc->valid) break;
+        if (!dsc->valid) {
+            if constexpr (kBlkChk) {
+                if (warp == kSumWarp) run_pending(&ctl->pend, lane);
+            }
+            break;
+        }
         const uint8_t *src = dsc->src;
         const uint32_t L = dsc->L;
 
@@ -258,6 +272,9 @@ __device__ __forceinline__ void fused_body(const Params &p) {
                     recs[sidx] = r;
                 }
                 have_claim = false;
+                if constexpr (kBlkChk) {
+                    if (warp == kSumWarp) run_pending(&ctl->pend, lane);  // (between two claims: no segment waits for this warp meanwhile)
+                }
             }
         }
         __syncthreads();
@@ -337,9 +354,10 @@ __device__ __forceinline__ void fused_body(const Params &p) {
                 csize = total + 1 + last + (last >= 15 ? (last - 15) / 255 + 1 : 0);
             }
             if (lane == 0) {
-                const BlockPlace pl = place_block(p, *dsc, csize, L);
+                const BlockPlace pl = place_block<kBlkChk>(p, *dsc, csize, L);
                 ctl->raw = pl.raw;
                 ctl->data = pl.data;
+                if constexpr (kBlkChk) ctl->size = pl.raw ? L : csize;
             }
         }
         __syncthreads();
@@ -366,27 +384,38 @@ __device__ __forceinline__ void fused_body(const Params &p) {
                     emit_seq(out, ctl->tail_off, src, L - ll, ll, 0, 0, lane);
                 }
             }
+            if constexpr (kBlkChk) {
+                if (warp == kSumWarp) {
+                    run_pending(&ctl->pend, lane);  // (still pending only when this block had no segment to parse)
+                    set_pending(&ctl->pend, out, ctl->size, lane);
+                }
+            }
         }
     }
 }
 
-__global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) { fused_body<false>(p); }
+__global__ void __launch_bounds__(kThreads, 2) sky_fused_kernel(const Params p) { fused_body<false, false>(p); }
 // SKY_F_CHECKSUM: the same kernel with the content checksum computed by the MD5 lanes (sky_checksum_kernel writes it).
-__global__ void __launch_bounds__(kThreads, 2) sky_fused_xxh_kernel(const Params p) { fused_body<true>(p); }
+__global__ void __launch_bounds__(kThreads, 2) sky_fused_xxh_kernel(const Params p) { fused_body<true, false>(p); }
+// SKY_F_BLOCK_CHECKSUM, without and with SKY_F_CHECKSUM: frames with LZ4's block checksums.
+__global__ void __launch_bounds__(kThreads, 2) sky_fused_bc_kernel(const Params p) { fused_body<false, true>(p); }
+__global__ void __launch_bounds__(kThreads, 2) sky_fused_xxh_bc_kernel(const Params p) { fused_body<true, true>(p); }
 
-// SKY_F_CHECKSUM epilogue, one thread per chunk, after the compressor has finished the frame: FLG gains C.Checksum
-// (0x68 -> 0x6C, 0x60 -> 0x64 for an empty chunk), the header checksum byte follows, and the XXH32 of the chunk goes
-// behind the EndMark.
-__global__ void sky_checksum_kernel(const ChunkDesc *chunks, const uint32_t *xxh, uint64_t *out_len, uint32_t n) {
+// Frame-descriptor epilogue, one thread per chunk, after the compressor has finished the frame: FLG gains `flg`
+// (SKY_F_CHECKSUM: C.Checksum 0x04, SKY_F_BLOCK_CHECKSUM: B.Checksum 0x10; 0x68 -> 0x6C / 0x78 / 0x7C, 0x60 -> 0x64 /
+// 0x70 / 0x74 for an empty chunk) and the header checksum byte follows.  With the content checksum (xxh != null) the
+// XXH32 of the chunk goes behind the EndMark.
+__global__ void sky_checksum_kernel(const ChunkDesc *chunks, const uint32_t *xxh, uint64_t *out_len, uint32_t n, uint32_t flg) {
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= n) return;
     const ChunkDesc cd = chunks[c];
     uint8_t *f = cd.dst;
     const uint32_t dlen = cd.len ? 10u : 2u;  // FLG, BD (+ content size)
-    f[4] |= 0x04;
+    f[4] |= (uint8_t)flg;
     uint8_t d[10];
     for (uint32_t i = 0; i < dlen; i++) d[i] = f[4 + i];
     f[4 + dlen] = (uint8_t)(xxh32_small(d, dlen) >> 8);
+    if (!xxh) return;
     const uint64_t end = out_len[c];
     const uint32_t x = xxh[c];
     f[end] = (uint8_t)x; f[end + 1] = (uint8_t)(x >> 8); f[end + 2] = (uint8_t)(x >> 16); f[end + 3] = (uint8_t)(x >> 24);
@@ -605,6 +634,11 @@ static const HcKernel kHcKernels[] = {sky_hc_kernel<hc_depth(3)>, sky_hc_kernel<
                                       sky_hc_kernel<hc_depth(6)>, sky_hc_kernel<hc_depth(7)>, sky_hc_kernel<hc_depth(8)>,
                                       sky_hc_kernel<hc_depth(9)>};
 static_assert(sizeof(kHcKernels) / sizeof(kHcKernels[0]) == kHcMaxLevel - kHcMinLevel + 1, "one HC kernel per level");
+// ... and with block checksums (SKY_F_BLOCK_CHECKSUM)
+static const HcKernel kHcBcKernels[] = {sky_hc_bc_kernel<hc_depth(3)>, sky_hc_bc_kernel<hc_depth(4)>, sky_hc_bc_kernel<hc_depth(5)>,
+                                        sky_hc_bc_kernel<hc_depth(6)>, sky_hc_bc_kernel<hc_depth(7)>, sky_hc_bc_kernel<hc_depth(8)>,
+                                        sky_hc_bc_kernel<hc_depth(9)>};
+static_assert(sizeof(kHcBcKernels) == sizeof(kHcKernels), "one HC kernel with block checksums per level");
 constexpr uint32_t kHcLevelShift = 8, kHcLevelMask = 0xfu << kHcLevelShift;  // SKY_F_HC_LEVEL's field in `flags`
 static_assert(SKY_F_HC_LEVEL(1) == (SKY_F_HC | (1u << kHcLevelShift)), "the level field of include/skychunk.h");
 // The level a batch's flags select: the level field, or kHcDefaultLevel when it is 0.
@@ -857,7 +891,13 @@ int sky_ctx_create(int device, uint64_t max_batch_bytes, uint32_t max_chunks, ui
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_xxh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_xxh_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    for (const auto k : {sky_fused_bc_kernel, sky_fused_xxh_bc_kernel}) {
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    }
     for (const HcKernel k : kHcKernels)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
+    for (const HcKernel k : kHcBcKernels)
         if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
     if (e != cudaSuccess) {
         g_err = ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (this build carries sm_90a code only)";
@@ -973,15 +1013,18 @@ static uint32_t fill_md5_order(uint32_t *order, uint32_t n, const uint64_t *len)
     return ng;
 }
 
-// SKY_F_HC selects how frames are made and SKY_F_CHECKSUM adds to the frame, so each needs SKY_F_LZ4, or no stage bit at
-// all (= LZ4 + MD5).  A level field needs SKY_F_HC and a level in kHcMinLevel .. kHcMaxLevel.
+// SKY_F_HC selects how frames are made and SKY_F_CHECKSUM / SKY_F_BLOCK_CHECKSUM add to the frame, so each needs
+// SKY_F_LZ4, or no stage bit at all (= LZ4 + MD5).  A level field needs SKY_F_HC and a level in kHcMinLevel .. kHcMaxLevel.
 static bool frame_flags_valid(uint32_t flags) {
     if ((flags & kHcLevelMask) && (!(flags & SKY_F_HC) || hc_level(flags) < kHcMinLevel || hc_level(flags) > kHcMaxLevel))
         return false;
-    return !(flags & (SKY_F_HC | SKY_F_CHECKSUM)) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5;
+    return !(flags & (SKY_F_HC | SKY_F_CHECKSUM | SKY_F_BLOCK_CHECKSUM)) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5;
 }
-// Bytes a chunk's frame may take: SKY_F_CHECKSUM adds the 4-byte content checksum behind the EndMark.
-static uint64_t frame_need(uint64_t n, uint32_t flags) { return sky_frame_bound(n) + ((flags & SKY_F_CHECKSUM) ? 4 : 0); }
+// Bytes a chunk's frame may take: SKY_F_CHECKSUM adds the 4-byte content checksum behind the EndMark,
+// SKY_F_BLOCK_CHECKSUM 4 bytes behind every block.
+static uint64_t frame_need(uint64_t n, uint32_t flags) {
+    return sky_frame_bound(n) + ((flags & SKY_F_CHECKSUM) ? 4 : 0) + ((flags & SKY_F_BLOCK_CHECKSUM) ? 4 * ((n + kBlock - 1) / kBlock) : 0);
+}
 
 // Fills the slot's metadata for a batch and enqueues: meta H2D, counter reset, fused kernel, results D2H.
 // `meta_st`: stream the three small metadata copies ride on (the H2D stream on the host path, so they are
@@ -990,7 +1033,7 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
                         const uint64_t *src_off, const uint64_t *src_len, uint8_t *d_dst, const uint64_t *dst_off, uint32_t flags) {
     if ((flags & (SKY_F_LZ4 | SKY_F_MD5)) == 0) flags |= SKY_F_LZ4 | SKY_F_MD5;
     if (flags & SKY_F_CHECKSUM) flags |= SKY_F_MD5;  // the content checksum comes from the MD5 lanes
-    const bool xxh = (flags & SKY_F_CHECKSUM) != 0;
+    const bool xxh = (flags & SKY_F_CHECKSUM) != 0, bc = (flags & SKY_F_BLOCK_CHECKSUM) != 0;
     if (flags & SKY_F_HC) {
         const int hrc = alloc_hc(ctx, s.hc);
         if (hrc != SKY_OK) return hrc;
@@ -1052,17 +1095,18 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
             ctx->launches++;
         }
         p.scratch = h.scratch;
-        kHcKernels[hc_level(flags) - kHcMinLevel]<<<ctx->sm_count, kHcThreads, kHcSmemBytes, st>>>(p);
+        (bc ? kHcBcKernels : kHcKernels)[hc_level(flags) - kHcMinLevel]<<<ctx->sm_count, kHcThreads, kHcSmemBytes, st>>>(p);
         CK(ctx, cudaGetLastError());
         if (md5) CK(ctx, cudaStreamWaitEvent(st, h.ev_join, 0));
     } else {
-        if (xxh) sky_fused_xxh_kernel<<<grid, kThreads, kSmemBytes, st>>>(p);
-        else sky_fused_kernel<<<grid, kThreads, kSmemBytes, st>>>(p);
+        void (*const k)(const Params) = bc ? (xxh ? sky_fused_xxh_bc_kernel : sky_fused_bc_kernel) : (xxh ? sky_fused_xxh_kernel : sky_fused_kernel);
+        k<<<grid, kThreads, kSmemBytes, st>>>(p);
         CK(ctx, cudaGetLastError());
     }
     ctx->launches++;
-    if (xxh) {
-        sky_checksum_kernel<<<(n + 127) / 128, 128, 0, st>>>(m.d_desc, m.xxh, m.outlen.d, n);
+    if (xxh || bc) {  // FLG and the header checksum byte of every frame, and the content checksum
+        sky_checksum_kernel<<<(n + 127) / 128, 128, 0, st>>>(m.d_desc, xxh ? (const uint32_t *)m.xxh : nullptr, m.outlen.d, n,
+                                                             (xxh ? 0x04u : 0u) | (bc ? 0x10u : 0u));
         CK(ctx, cudaGetLastError());
         ctx->launches++;
     }

@@ -58,12 +58,14 @@ def run_stream(
     high_ratio: bool = False,
     content_checksum: bool = False,
     compression_level: Optional[int] = None,
+    block_checksum: bool = False,
 ) -> Dict:
     """Stream ``n_requests`` chunk requests (recycling ``pool_files`` by hard link) through the operator.
 
     The first ``warmup_requests`` completions are not timed (worker start-up: CUDA context, pinned staging).
-    ``high_ratio``, ``content_checksum`` and ``compression_level`` are handed to the operator (GatewayCompressHash's
-    high-ratio frames, frames with LZ4's content checksum, the high-ratio level) when set.
+    ``high_ratio``, ``content_checksum``, ``compression_level`` and ``block_checksum`` are handed to the operator
+    (GatewayCompressHash's high-ratio frames, frames with LZ4's content checksum, the high-ratio level, frames with LZ4's
+    block checksums) when set.
     Returns {"wall_s", "bytes", "records": [{chunk_id, pool_index, md5, raw_len, frame_path}], "status": {...}}.
     """
     chunk_dir = Path(chunk_dir)
@@ -77,6 +79,7 @@ def run_stream(
         **({"high_ratio": True} if high_ratio else {}),
         **({"content_checksum": True} if content_checksum else {}),
         **({"compression_level": compression_level} if compression_level is not None else {}),
+        **({"block_checksum": True} if block_checksum else {}),
     )
     op.start_workers()
     records: List[Dict] = []

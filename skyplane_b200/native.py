@@ -14,8 +14,9 @@ LIB_PATH = _PKG / "libskychunk.so"
 
 SKY_OK = 0
 SKY_E_INVALID, SKY_E_NOGPU, SKY_E_CUDA, SKY_E_CAPACITY, SKY_E_BUSY, SKY_E_TICKET, SKY_E_NOMEM, SKY_E_NOKEY = -1, -2, -3, -4, -5, -6, -7, -8
-F_LZ4, F_MD5, F_E2EE, F_HC, F_CHECKSUM = 1, 2, 16, 32, 64
-CHECKSUM_BYTES = 4  # F_CHECKSUM: the content checksum (u32le XXH32) behind the EndMark
+F_LZ4, F_MD5, F_E2EE, F_HC, F_CHECKSUM, F_BLOCK_CHECKSUM = 1, 2, 16, 32, 64, 128
+CHECKSUM_BYTES = 4  # F_CHECKSUM: the content checksum (u32le XXH32) behind the EndMark; F_BLOCK_CHECKSUM: as many per block
+BLOCK_BYTES = 65536
 # SKY_F_HC_LEVEL(l): the high-ratio level l (3..9: 2**(l - 1) chain candidates per position) in bits 8..11 of the flags;
 # a level field of 0 with F_HC is the default level
 HC_LEVEL_SHIFT = 8
@@ -176,6 +177,13 @@ def hc_flags(level: Optional[int] = None, hc: bool = False, compress: bool = Tru
 
 def frame_bound(n: int) -> int:
     return int(lib().sky_frame_bound(n))
+
+
+def frame_need(n: int, checksum: bool = False, block_checksum: bool = False) -> int:
+    """Bytes an n-byte chunk's frame may take (dst_cap before any SecretBox): frame_bound(n), + 4 for the content checksum,
+    + 4 per 64 KiB block for block checksums -- what sky_submit / sky_process_device require."""
+    blocks = -(-n // BLOCK_BYTES)
+    return frame_bound(n) + (CHECKSUM_BYTES if checksum else 0) + (CHECKSUM_BYTES * blocks if block_checksum else 0)
 
 
 def round16(x: int) -> int:

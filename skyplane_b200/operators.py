@@ -136,6 +136,7 @@ class GatewayCompressHash(GatewayOperator):
         high_ratio: bool = False,
         content_checksum: bool = False,
         compression_level: Optional[int] = None,
+        block_checksum: bool = False,
     ):
         """use_compression / e2ee_key_bytes: GatewaySender's arguments of the same name (gateway_operator.py:154-168):
         ``use_compression=False`` digests the chunk and lets it pass through uncompressed (``is_compressed=False``);
@@ -148,6 +149,8 @@ class GatewayCompressHash(GatewayOperator):
         compression_level: python-lz4's argument of the same name (``ChunkStage.launch(level=...)``): 3..9 makes the
         frames with the high-ratio parse at that level (2**(level - 1) chain candidates per position, more ratio for more GPU
         time), 0..2 with the fast compressor; ``high_ratio`` alone means level 5.  Needs ``use_compression``.
+        block_checksum: every block of the frame carries LZ4's block checksum (XXH32 of the block as stored, python-lz4's
+        argument of the same name), so any LZ4 decoder rejects a damaged block before decoding it.  Needs ``use_compression``.
         sink: ``callable(worker_id) -> socket``, called once in each worker.  With a sink the worker sends every payload
         straight from the pinned staging slot (``wire.send_results``: WireProtocolHeader + payload, no intermediate bytes
         object, no frame file) -- the tail of ``GatewaySender.process`` (gateway_operator.py:367-402)."""
@@ -159,6 +162,9 @@ class GatewayCompressHash(GatewayOperator):
         if content_checksum and not self.use_compression:
             raise ValueError("content_checksum is carried by the LZ4 frame: it needs use_compression")
         self.content_checksum = bool(content_checksum)
+        if block_checksum and not self.use_compression:
+            raise ValueError("block_checksum is carried by the LZ4 frame: it needs use_compression")
+        self.block_checksum = bool(block_checksum)
         from skyplane_b200 import native
 
         native.hc_flags(compression_level, self.high_ratio, self.use_compression)  # (ValueError on a bad level, here and not in a worker)
@@ -310,6 +316,8 @@ class GatewayCompressHash(GatewayOperator):
             opts["checksum"] = True
         if self.compression_level is not None:
             opts["level"] = self.compression_level
+        if self.block_checksum:
+            opts["block_checksum"] = True
         stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None, **opts)
         return True
 

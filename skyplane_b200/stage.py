@@ -36,9 +36,10 @@ class StageResult:
 
 
 def _out_room(n: int) -> int:
-    """Staging bytes an n-byte chunk's payload may take: its frame with the content checksum (launch(checksum=True)),
-    sealed in a SecretBox (encrypt=True).  Reserved whatever the batch is launched with."""
-    return native.round16(native.frame_bound(n) + native.CHECKSUM_BYTES + native.BOX_OVERHEAD)
+    """Staging bytes an n-byte chunk's payload may take: its frame with the content and block checksums
+    (launch(checksum=True, block_checksum=True)), sealed in a SecretBox (encrypt=True).  Reserved whatever the batch is
+    launched with."""
+    return native.round16(native.frame_need(n, checksum=True, block_checksum=True) + native.BOX_OVERHEAD)
 
 
 class _Slot:
@@ -79,6 +80,10 @@ class ChunkStage:
         self.max_batch_bytes = max_batch_bytes
         in_bytes = native.round16(max_batch_bytes) + 16 * max_chunks
         out_bytes = max_batch_bytes + 4 * (max_batch_bytes // 65536 + 1) + 128 * max_chunks
+        # block checksums: 4 bytes per block of every chunk (the chunks' blocks number at most in_bytes / 64 KiB + 1 +
+        # max_chunks), and up to 12 more per chunk where rounding to 16 bytes took them before -- so every batch that fits
+        # without them still fits
+        out_bytes += native.CHECKSUM_BYTES * (in_bytes // native.BLOCK_BYTES + 1) + 16 * max_chunks
         self._slots = [_Slot(in_bytes, out_bytes) for _ in range(n_slots)]
         self._free = list(self._slots)
 
@@ -157,11 +162,13 @@ class ChunkStage:
         self._has_key = key is not None
 
     def launch(self, slot: _Slot, compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None, hc: bool = False,
-               checksum: bool = False, level: Optional[int] = None) -> _Slot:
+               checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False) -> _Slot:
         """compress=False is the reference's `compress: false` (digest only, the chunk passes through);
         encrypt=True seals every payload with the stage's key (nonces: 24 bytes per chunk, default os.urandom);
         hc=True makes the frames with the high-ratio parse (F_HC): same frame format, fewer bytes, more GPU time;
         checksum=True gives every frame LZ4's content checksum (F_CHECKSUM), which any LZ4 decoder verifies;
+        block_checksum=True gives every block of the frame LZ4's block checksum (F_BLOCK_CHECKSUM), which any LZ4 decoder
+        verifies before it decodes the block;
         level is python-lz4's compression_level: 3..9 runs the high-ratio parse at that level (2**(level - 1) chain
         candidates per position: more ratio for more GPU time), hc=True alone means level 5, 0..2 is the fast path."""
         if not slot.lens:
@@ -170,6 +177,8 @@ class ChunkStage:
             raise ValueError("hc=True selects how frames are compressed: it needs compress=True")
         if checksum and not compress:
             raise ValueError("checksum=True is carried by the LZ4 frame: it needs compress=True")
+        if block_checksum and not compress:
+            raise ValueError("block_checksum=True is carried by the LZ4 frame: it needs compress=True")
         hc_bits = native.hc_flags(level, hc, compress)
         if hc_bits and not native.kernel_config()["hc_depth"]:
             raise native.SkyChunkError(native.SKY_E_INVALID, f"{native.LIB_PATH.name} was built without the high-ratio kernel (F_HC)")
@@ -178,13 +187,13 @@ class ChunkStage:
         base_in, base_out = slot.inp.addr, slot.out.addr
         src = [base_in + o for o in slot.in_off]
         flags = (native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0) | hc_bits
-                 | (native.F_CHECKSUM if checksum else 0))
+                 | (native.F_CHECKSUM if checksum else 0) | (native.F_BLOCK_CHECKSUM if block_checksum else 0))
         if encrypt and nonces is None:
             nonces = os.urandom(24 * len(slot.lens))  # what nacl.utils.random(24) draws per message
         if compress or encrypt:
             dst = [base_out + o for o in slot.out_off]
-            caps = [(native.frame_bound(n) + (native.CHECKSUM_BYTES if checksum else 0) if compress else n)
-                    + (native.BOX_OVERHEAD if encrypt else 0) for n in slot.lens]
+            caps = [(native.frame_need(n, checksum, block_checksum) if compress else n) + (native.BOX_OVERHEAD if encrypt else 0)
+                    for n in slot.lens]
         else:
             dst = caps = None
         slot.flags = flags
@@ -204,10 +213,12 @@ class ChunkStage:
 
     # ------------------------------------------------------------------ sync convenience
     def process(self, chunks: Sequence[BytesLike], compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None,
-                hc: bool = False, checksum: bool = False, level: Optional[int] = None) -> List[StageResult]:
+                hc: bool = False, checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False) -> List[StageResult]:
         """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes (hc, checksum,
-        level: see launch)."""
+        level, block_checksum: see launch)."""
         native.hc_flags(level, hc, compress)  # (bad arguments fail before the first batch)
+        if block_checksum and not compress:
+            raise ValueError("block_checksum=True is carried by the LZ4 frame: it needs compress=True")
         out: List[StageResult] = []
         i = 0
         while i < len(chunks):
@@ -219,7 +230,7 @@ class ChunkStage:
             if j == i:
                 self.release(slot)
                 raise native.SkyChunkError(native.SKY_E_CAPACITY, f"chunk of {memoryview(chunks[i]).nbytes} bytes exceeds max_batch_bytes")
-            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum, level)
+            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum, level, block_checksum)
             for r in self.collect(slot):
                 out.append(StageResult(frame=memoryview(bytes(r.frame)), md5=r.md5, raw_len=r.raw_len, comp_len=r.comp_len,
                                        is_compressed=r.is_compressed, is_encrypted=r.is_encrypted))

@@ -52,8 +52,8 @@ def blocks(data: bytes, o: Opts):
     return out
 
 
-def frame(data: bytes, o: Opts | None = None) -> bytes:
-    return tile_model.assemble(len(data), blocks(data, o or kernel_opts()))
+def frame(data: bytes, o: Opts | None = None, block_checksum: bool = False) -> bytes:
+    return tile_model.assemble(len(data), blocks(data, o or kernel_opts()), block_checksum)
 
 
 def liblz4_frame(data: bytes, level: int, linked: bool = False, content_checksum: bool = False, block_checksum: bool = False) -> bytes:

@@ -3,7 +3,9 @@
 Writes one JSON line per configuration.  Used to fill profiles/ and DESIGN.md tables; not a bench line.
 Flag sets: lz4, md5, both (the fused kernel), hc (SKY_F_HC: high-ratio frames + MD5), hc-lz4 (high-ratio frames only),
 checksum / hc-checksum (SKY_F_CHECKSUM: frames with LZ4's content checksum, fast or high-ratio), hc3 .. hc9 and
-hc3-checksum .. hc9-checksum (SKY_F_HC_LEVEL(3..9): the high-ratio mode at that level; hc5 makes hc's frames).
+hc3-checksum .. hc9-checksum (SKY_F_HC_LEVEL(3..9): the high-ratio mode at that level; hc5 makes hc's frames);
+block-checksum, block-checksum-checksum, hc-block-checksum, hc-block-checksum-checksum and hc3-block-checksum ..
+hc9-block-checksum (SKY_F_BLOCK_CHECKSUM: the same frames with LZ4's block checksums, alone or with the content checksum).
 --decode-from liblz4[-linked][-checksums] times the receiver on liblz4's level-0 frames made on the host from the same
 input: independent or linked blocks, without checksums or with block and content checksums.
 --ref-ratio adds the reference's ratio (liblz4 level 0, linked blocks) on the distinct chunks; --liblz4-level9 times liblz4
@@ -113,6 +115,10 @@ def main():
     for lv in range(native.HC_MIN_LEVEL, native.HC_MAX_LEVEL + 1):
         FL[f"hc{lv}"] = native.hc_level_flag(lv)
         FL[f"hc{lv}-checksum"] = native.hc_level_flag(lv) | native.F_CHECKSUM
+        FL[f"hc{lv}-block-checksum"] = native.hc_level_flag(lv) | native.F_BLOCK_CHECKSUM
+    FL.update({"block-checksum": native.F_BLOCK_CHECKSUM, "block-checksum-checksum": native.F_BLOCK_CHECKSUM | native.F_CHECKSUM,
+               "hc-block-checksum": native.F_HC | native.F_BLOCK_CHECKSUM,
+               "hc-block-checksum-checksum": native.F_HC | native.F_BLOCK_CHECKSUM | native.F_CHECKSUM})
     for wl in a.workloads.split(","):
         for sz in a.sizes_mib.split(","):
             chunk_bytes = int(float(sz) * (1 << 20))
@@ -129,8 +135,8 @@ def main():
                     row.update(liblz4_level9_all_cores(chunks))
                 print(json.dumps(row), flush=True)
             d_in, stride = make_input(wl, n, chunk_bytes, dev)
-            bound = native.frame_bound(chunk_bytes) + native.CHECKSUM_BYTES  # (room for a content checksum)
-            so = native.round16(bound + 4 * (chunk_bytes // 65536 + 1))  # (and for liblz4's block checksums, --decode-from)
+            bound = native.frame_need(chunk_bytes, checksum=True, block_checksum=True)  # (room for content and block checksums)
+            so = native.round16(bound)
             d_out = torch.empty(n * so + 64, dtype=torch.uint8, device=dev)
             ctx = native.Context(0, n * stride, n, 0)
             src_off = [i * stride for i in range(n)]

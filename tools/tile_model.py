@@ -68,17 +68,28 @@ def blocks(data: bytes, o: Opts):
     return out
 
 
-def assemble(n: int, blks) -> bytes:
-    """The stage's frame around an n-byte chunk's blocks [(compressed size or 0 when stored raw, block bytes)]."""
+def assemble(n: int, blks, block_checksum: bool = False) -> bytes:
+    """The stage's frame around an n-byte chunk's blocks [(compressed size or 0 when stored raw, block bytes)];
+    block_checksum (SKY_F_BLOCK_CHECKSUM): FLG's B.Checksum bit, and u32le XXH32 of every block's bytes behind them."""
+    flg = 0x10 if block_checksum else 0
     if not n:
-        d = bytes([0x60, 0x40])
+        d = bytes([0x60 | flg, 0x40])
         return bytes([0x04, 0x22, 0x4D, 0x18]) + d + bytes([(_xxh32_small(d) >> 8) & 0xFF]) + bytes(4)
-    d = bytes([0x68, 0x40]) + n.to_bytes(8, "little")
+    d = bytes([0x68 | flg, 0x40]) + n.to_bytes(8, "little")
     fr = bytearray(bytes([0x04, 0x22, 0x4D, 0x18]) + d + bytes([(_xxh32_small(d) >> 8) & 0xFF]))
     for c, b in blks:
         fr += (c if c else (len(b) | 0x80000000)).to_bytes(4, "little") + b
+        if block_checksum:
+            fr += xxh32(b).to_bytes(4, "little")
     return bytes(fr + bytes(4))
 
 
-def frame(data: bytes, o: Opts | None = None) -> bytes:
-    return assemble(len(data), blocks(data, o or kernel_opts()))
+def xxh32(b: bytes) -> int:
+    """XXH32 (seed 0) of any input, from the project's C oracle."""
+    import oracle
+
+    return oracle.xxh32(b)
+
+
+def frame(data: bytes, o: Opts | None = None, block_checksum: bool = False) -> bytes:
+    return assemble(len(data), blocks(data, o or kernel_opts()), block_checksum)
