@@ -90,6 +90,16 @@ extern "C" {
  * SKY_F_LZ4 (no frame to carry them) it is SKY_E_INVALID.  The compressor CTA that writes a block hashes it; one more
  * launch per batch writes FLG and the header checksum byte. */
 #define SKY_F_BLOCK_CHECKSUM 128u
+/* frame verification (sky_submit, with any of the frame flags above and SKY_F_E2EE): before a batch's frames are sealed
+ * or copied out, the GPU checks every frame against its chunk -- header exactly as the stage writes it, block words,
+ * block and content checksums, and every block decoded against the chunk's bytes under liblz4's rules -- so that a frame
+ * the stage returns restores its chunk under any LZ4 decoder.  A frame that fails is rewritten in place as the chunk's
+ * stored-block frame (same header and checksum flags, every block stored raw; sky_frame_bound plus the checksum bytes,
+ * which dst_cap already holds) and its status (sky_wait_verify) is the failing check's SKY_D_* code.  Alone it means
+ * LZ4 + MD5 + verify; without SKY_F_LZ4 (no frame) it is SKY_E_INVALID, and sky_process_device does not take it
+ * (sky_verify_device runs the same check over frames in HBM).  Three more launches per batch.  It sits outside the
+ * SKY_F_HC_LEVEL field. */
+#define SKY_F_VERIFY 4096u
 
 typedef struct sky_ctx sky_ctx;
 
@@ -137,6 +147,10 @@ SKY_API int sky_pinned_free(void *p);
 SKY_API int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t *src_len, void *const *dst,
                const uint64_t *dst_cap, uint32_t flags, const uint8_t *nonces, uint64_t *ticket);
 SKY_API int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, float *kernel_ms);
+/* sky_wait, plus verify[n]: per chunk 0 (the frame restores the chunk) or the SKY_D_* code of the frame as the compressor
+ * made it, whose payload is now the stored-block frame.  verify != NULL needs a ticket submitted with SKY_F_VERIFY
+ * (SKY_E_INVALID otherwise, and the ticket stays un-waited); sky_wait also completes such a ticket. */
+SKY_API int sky_wait_verify(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, float *kernel_ms);
 SKY_API int sky_set_e2ee_key(sky_ctx *ctx, const uint8_t *key32);
 SKY_API uint64_t sky_box_bound(uint64_t n); /* sky_frame_bound(n) + SKY_BOX_OVERHEAD */
 
@@ -171,11 +185,26 @@ SKY_API int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, cons
 #define SKY_D_TRUNCATED (-6)
 #define SKY_D_AUTH (-7) /* SKY_F_E2EE: the box's Poly1305 tag does not verify (nacl.exceptions.CryptoError in the reference) */
 #define SKY_D_CHECKSUM (-8) /* a block checksum or the content checksum (XXH32) does not match: lz4.frame.decompress raises */
+#define SKY_D_MISMATCH (-9) /* SKY_F_VERIFY: the frame is well formed but decodes to other bytes than the chunk */
 SKY_API int sky_decode_device(sky_ctx *ctx, uint32_t n, const void *d_frames, const uint64_t *frame_off, const uint64_t *frame_len,
                       void *d_out, const uint64_t *out_off, const uint64_t *raw_len, void *stream, int32_t *status, uint8_t *md5,
                       float *kernel_ms);
 SKY_API int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64_t *frame_len, void *const *dst,
                const uint64_t *raw_len, uint32_t flags, int32_t *status, uint8_t *md5, float *kernel_ms);
+
+/* ---- frame verification over frames in HBM (SKY_F_VERIFY's check and repair) -----------------------------------------
+ * Chunk i is d_src[src_off[i] .. +src_len[i]) (d_src and src_off multiples of 16, readable up to the next multiple of 16),
+ * its frame d_frames[frame_off[i] .. +frame_len[i]) (any alignment, readable up to the next multiple of 4 bytes).  flags:
+ * the frame flags the frames were made with (SKY_F_CHECKSUM, SKY_F_BLOCK_CHECKSUM fix FLG and the trailer; the stage
+ * and compressor bits are accepted as sky_submit takes them; SKY_F_E2EE or SKY_F_MD5 alone is SKY_E_INVALID).
+ * content_xxh[i]: the chunk's XXH32, given exactly when SKY_F_CHECKSUM is set.  status[i] = 0 or the SKY_D_* code of the
+ * check that failed.  frame_cap == NULL: check only, no byte changes.  Otherwise every failing frame is rewritten in place
+ * as its stored-block frame, frame_len[i] becomes its length, and nothing outside [frame, frame + frame_cap[i]) is written;
+ * frame_cap[i] < sky_frame_bound(src_len[i]) + the flags' checksum bytes is SKY_E_CAPACITY.  Synchronous; kernel_ms =
+ * device time of the check (and repair).  Uses slot 0's metadata, as sky_process_device does. */
+SKY_API int sky_verify_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64_t *src_off, const uint64_t *src_len, void *d_frames,
+                      const uint64_t *frame_off, uint64_t *frame_len, const uint64_t *frame_cap, const uint32_t *content_xxh,
+                      uint32_t flags, void *stream, int32_t *status, float *kernel_ms);
 
 /* Device-memory helpers so a host without torch can drive the device path. */
 SKY_API int sky_device_alloc(sky_ctx *ctx, uint64_t bytes, void **dptr);

@@ -184,4 +184,23 @@ __device__ __forceinline__ void set_pending(PendingChecksum *pc, uint8_t *data, 
     }
 }
 
+// Frame-descriptor epilogue of chunk c's finished frame, one thread: FLG gains `flg` (SKY_F_CHECKSUM: C.Checksum 0x04,
+// SKY_F_BLOCK_CHECKSUM: B.Checksum 0x10; 0x68 -> 0x6C / 0x78 / 0x7C, 0x60 -> 0x64 / 0x70 / 0x74 for an empty chunk) and
+// the header checksum byte follows.  With the content checksum (xxh != null) xxh[c], the XXH32 of the chunk, goes behind
+// the EndMark at out_len[c], which grows by 4.
+__device__ __forceinline__ void finish_frame(const ChunkDesc *chunks, const uint32_t *xxh, uint64_t *out_len, uint32_t c, uint32_t flg) {
+    const ChunkDesc cd = chunks[c];
+    uint8_t *f = cd.dst;
+    const uint32_t dlen = cd.len ? 10u : 2u;  // FLG, BD (+ content size)
+    f[4] |= (uint8_t)flg;
+    uint8_t d[10];
+    for (uint32_t i = 0; i < dlen; i++) d[i] = f[4 + i];
+    f[4 + dlen] = (uint8_t)(xxh32_small(d, dlen) >> 8);
+    if (!xxh) return;
+    const uint64_t end = out_len[c];
+    const uint32_t x = xxh[c];
+    f[end] = (uint8_t)x; f[end + 1] = (uint8_t)(x >> 8); f[end + 2] = (uint8_t)(x >> 16); f[end + 3] = (uint8_t)(x >> 24);
+    out_len[c] = end + 4;
+}
+
 }  // namespace sky

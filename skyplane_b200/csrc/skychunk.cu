@@ -40,6 +40,7 @@
 #include "lz4.cuh"
 #include "lz4dec.cuh"
 #include "lz4hc.cuh"
+#include "lz4verify.cuh"
 #include "md5.cuh"
 #include "secretbox.cuh"
 
@@ -401,25 +402,11 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_xxh_kernel(const Params
 __global__ void __launch_bounds__(kThreads, 2) sky_fused_bc_kernel(const Params p) { fused_body<false, true>(p); }
 __global__ void __launch_bounds__(kThreads, 2) sky_fused_xxh_bc_kernel(const Params p) { fused_body<true, true>(p); }
 
-// Frame-descriptor epilogue, one thread per chunk, after the compressor has finished the frame: FLG gains `flg`
-// (SKY_F_CHECKSUM: C.Checksum 0x04, SKY_F_BLOCK_CHECKSUM: B.Checksum 0x10; 0x68 -> 0x6C / 0x78 / 0x7C, 0x60 -> 0x64 /
-// 0x70 / 0x74 for an empty chunk) and the header checksum byte follows.  With the content checksum (xxh != null) the
-// XXH32 of the chunk goes behind the EndMark.
+// Frame-descriptor epilogue (finish_frame, frame.cuh), one thread per chunk, after the compressor has finished the frame.
 __global__ void sky_checksum_kernel(const ChunkDesc *chunks, const uint32_t *xxh, uint64_t *out_len, uint32_t n, uint32_t flg) {
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= n) return;
-    const ChunkDesc cd = chunks[c];
-    uint8_t *f = cd.dst;
-    const uint32_t dlen = cd.len ? 10u : 2u;  // FLG, BD (+ content size)
-    f[4] |= (uint8_t)flg;
-    uint8_t d[10];
-    for (uint32_t i = 0; i < dlen; i++) d[i] = f[4 + i];
-    f[4 + dlen] = (uint8_t)(xxh32_small(d, dlen) >> 8);
-    if (!xxh) return;
-    const uint64_t end = out_len[c];
-    const uint32_t x = xxh[c];
-    f[end] = (uint8_t)x; f[end + 1] = (uint8_t)(x >> 8); f[end + 2] = (uint8_t)(x >> 16); f[end + 3] = (uint8_t)(x >> 24);
-    out_len[c] = end + 4;
+    finish_frame(chunks, xxh, out_len, c, flg);
 }
 
 
@@ -662,6 +649,14 @@ struct BoxArrays {  // E2EE: box slab, per-chunk box descriptors, stream-block p
     PinnedMem<uint8_t> h_nonce; DevMem<uint8_t> d_nonce;
     PinnedMem<int32_t> h_status; DevMem<int32_t> d_status;
 };
+struct VerifyArrays {  // SKY_F_VERIFY: block-table bases, statuses (device, and settled in mapped host memory), block table
+    PinnedMem<uint64_t> h_blk_base; DevMem<uint64_t> d_blk_base;
+    DevMem<int32_t> d_status;
+    Mapped<int32_t> status;
+    DevMem<uint32_t> d_counter;
+    DevMem<DecBlock> d_blocks;  // per block of the batch: blocks_cap entries, grown on demand
+    uint64_t blocks_cap = 0;
+};
 struct Ticket {  // the batch a slot has in flight on the host path
     bool busy = false, d2h_issued = false;
     uint64_t id = 0;
@@ -680,6 +675,7 @@ struct Slot {
     DecodeArrays dec;
     BoxArrays box;
     HcArrays hc;
+    VerifyArrays verify;
     Ticket ticket;
 };
 
@@ -771,6 +767,19 @@ static int alloc_hc(sky_ctx *ctx, HcArrays &h) {
     CK(ctx, cudaEventCreateWithFlags(a.ev_fork.put(), cudaEventDisableTiming));
     CK(ctx, cudaEventCreateWithFlags(a.ev_join.put(), cudaEventDisableTiming));
     h = std::move(a);
+    return SKY_OK;
+}
+
+static int alloc_verify(sky_ctx *ctx, VerifyArrays &v) {
+    if (v.d_status) return SKY_OK;
+    const size_t nc = ctx->max_chunks;
+    VerifyArrays a;
+    CK(ctx, cudaMallocHost(a.h_blk_base.put(), nc * sizeof(uint64_t)));
+    CK(ctx, cudaMalloc(a.d_blk_base.put(), nc * sizeof(uint64_t)));
+    CK(ctx, cudaMalloc(a.d_status.put(), nc * sizeof(int32_t)));
+    CK(ctx, a.status.alloc(nc));
+    CK(ctx, cudaMalloc(a.d_counter.put(), sizeof(uint32_t)));
+    v = std::move(a);
     return SKY_OK;
 }
 
@@ -1013,17 +1022,62 @@ static uint32_t fill_md5_order(uint32_t *order, uint32_t n, const uint64_t *len)
     return ng;
 }
 
-// SKY_F_HC selects how frames are made and SKY_F_CHECKSUM / SKY_F_BLOCK_CHECKSUM add to the frame, so each needs
-// SKY_F_LZ4, or no stage bit at all (= LZ4 + MD5).  A level field needs SKY_F_HC and a level in kHcMinLevel .. kHcMaxLevel.
+// SKY_F_HC selects how frames are made, SKY_F_CHECKSUM / SKY_F_BLOCK_CHECKSUM add to the frame and SKY_F_VERIFY checks
+// it, so each needs SKY_F_LZ4, or no stage bit at all (= LZ4 + MD5).  A level field needs SKY_F_HC and a level in kHcMinLevel .. kHcMaxLevel.
 static bool frame_flags_valid(uint32_t flags) {
     if ((flags & kHcLevelMask) && (!(flags & SKY_F_HC) || hc_level(flags) < kHcMinLevel || hc_level(flags) > kHcMaxLevel))
         return false;
-    return !(flags & (SKY_F_HC | SKY_F_CHECKSUM | SKY_F_BLOCK_CHECKSUM)) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5;
+    return !(flags & (SKY_F_HC | SKY_F_CHECKSUM | SKY_F_BLOCK_CHECKSUM | SKY_F_VERIFY)) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5;
 }
 // Bytes a chunk's frame may take: SKY_F_CHECKSUM adds the 4-byte content checksum behind the EndMark,
 // SKY_F_BLOCK_CHECKSUM 4 bytes behind every block.
 static uint64_t frame_need(uint64_t n, uint32_t flags) {
     return sky_frame_bound(n) + ((flags & SKY_F_CHECKSUM) ? 4 : 0) + ((flags & SKY_F_BLOCK_CHECKSUM) ? 4 * ((n + kBlock - 1) / kBlock) : 0);
+}
+
+// Enqueues the frame check (SKY_F_VERIFY, lz4verify.cuh) of the n chunks in the slot's batch metadata (h_desc / d_desc,
+// the frame lengths in outlen, the content checksums in xxh under SKY_F_CHECKSUM) on `st`: index, block check, settle.
+// flags: what the frames were made with (FLG, checksums); repair: rewrite every failing frame as its stored-block frame.
+// The settled statuses land in s.verify.status.
+static int launch_verify(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, uint32_t rows, uint32_t flags, bool repair) {
+    int rc = alloc_verify(ctx, s.verify);
+    if (rc != SKY_OK) return rc;
+    VerifyArrays &v = s.verify;
+    BatchMeta &m = s.meta;
+    uint64_t nblk_total = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        v.h_blk_base[i] = nblk_total;
+        nblk_total += m.h_desc[i].nblk;
+    }
+    if (nblk_total + 1 > v.blocks_cap) {
+        CK(ctx, cudaStreamSynchronize(st));  // an earlier check is done with the old table
+        v.blocks_cap = 0;
+        CK(ctx, cudaMalloc(v.d_blocks.put(), (nblk_total + 1) * sizeof(DecBlock)));
+        v.blocks_cap = nblk_total + 1;
+    }
+    CK(ctx, cudaMemcpyAsync(v.d_blk_base, v.h_blk_base, n * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaMemsetAsync(v.d_counter, 0, sizeof(uint32_t), st));
+    VerifyParams p;
+    p.chunks = m.d_desc;
+    p.frame_len = m.outlen.d;
+    p.xxh = (flags & SKY_F_CHECKSUM) ? (const uint32_t *)m.xxh : nullptr;
+    p.blk_base = v.d_blk_base;
+    p.blocks = v.d_blocks;
+    p.status = v.d_status;
+    p.status_out = v.status.d;
+    p.counter = v.d_counter;
+    p.n_chunks = n;
+    p.rows = rows;
+    p.flags = flags;
+    p.repair = repair ? 1u : 0u;
+    sky_verify_index_kernel<<<(n + 127) / 128, 128, 0, st>>>(p);
+    CK(ctx, cudaGetLastError());
+    sky_verify_kernel<<<ctx->sm_count * 2, kVerifyThreads, 0, st>>>(p);
+    CK(ctx, cudaGetLastError());
+    sky_verify_settle_kernel<<<n, kRepairWarps * 32, 0, st>>>(p);
+    CK(ctx, cudaGetLastError());
+    ctx->launches += 3;
+    return SKY_OK;
 }
 
 // Fills the slot's metadata for a batch and enqueues: meta H2D, counter reset, fused kernel, results D2H.
@@ -1110,6 +1164,10 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
         CK(ctx, cudaGetLastError());
         ctx->launches++;
     }
+    if (flags & SKY_F_VERIFY) {  // every frame is final here: check it, and repair it before it is sealed or copied out
+        rc = launch_verify(ctx, s, st, n, rows, flags, true);
+        if (rc != SKY_OK) return rc;
+    }
     CK(ctx, cudaEventRecord(s.ev_k1, st));
     if (flags & SKY_F_E2EE) {
         rc = launch_seal(ctx, s, st, n, d_dst, flags);
@@ -1150,7 +1208,7 @@ int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64
                        void *d_dst, const uint64_t *dst_off, const uint64_t *dst_cap, uint32_t flags, void *stream,
                        uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
     if (!ctx || n == 0 || !src_off || !src_len || !dst_off || !dst_cap || !d_dst) return SKY_E_INVALID;
-    if (flags & SKY_F_E2EE) return SKY_E_INVALID;  // boxes are a host-path feature (sky_submit)
+    if (flags & (SKY_F_E2EE | SKY_F_VERIFY)) return SKY_E_INVALID;  // host-path features (sky_submit; sky_verify_device checks)
     if (!frame_flags_valid(flags)) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
     if ((reinterpret_cast<uintptr_t>(d_src) & 15) || (reinterpret_cast<uintptr_t>(d_dst) & 15)) return SKY_E_INVALID;
@@ -1216,13 +1274,14 @@ int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t 
     return SKY_OK;
 }
 
-int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
+int sky_wait_verify(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, float *kernel_ms) {
     if (!ctx) return SKY_E_INVALID;
     Slot *sp = nullptr;
     for (Slot &s : ctx->slots)
         if (s.ticket.busy && s.ticket.id == ticket) { sp = &s; break; }
     if (!sp) return SKY_E_TICKET;
     Slot &s = *sp;
+    if (verify && !(s.ticket.flags & SKY_F_VERIFY)) return SKY_E_INVALID;  // (the ticket stays valid)
     CK(ctx, cudaSetDevice(ctx->device));
     { int prc = progress(ctx); if (prc != SKY_OK) return prc; }
     if (!s.ticket.d2h_issued) {
@@ -1234,8 +1293,51 @@ int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, flo
     CK(ctx, cudaEventSynchronize(s.ev_d2h));
     if (out_len) memcpy(out_len, s.meta.outlen.h, s.ticket.n * sizeof(uint64_t));
     if (md5) memcpy(md5, s.meta.md5.h, (size_t)s.ticket.n * 16);
+    if (verify) memcpy(verify, s.verify.status.h, s.ticket.n * sizeof(int32_t));
     if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, s.ev_k0, s.ev_k1));
     s.ticket.busy = false;
+    return SKY_OK;
+}
+
+int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
+    return sky_wait_verify(ctx, ticket, out_len, md5, nullptr, kernel_ms);
+}
+
+int sky_verify_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64_t *src_off, const uint64_t *src_len, void *d_frames,
+                      const uint64_t *frame_off, uint64_t *frame_len, const uint64_t *frame_cap, const uint32_t *content_xxh,
+                      uint32_t flags, void *stream, int32_t *status, float *kernel_ms) {
+    if (!ctx || n == 0 || !src_off || !src_len || !d_frames || !frame_off || !frame_len) return SKY_E_INVALID;
+    if ((flags & SKY_F_E2EE) || !frame_flags_valid(flags) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) == SKY_F_MD5) return SKY_E_INVALID;
+    if (((flags & SKY_F_CHECKSUM) != 0) != (content_xxh != nullptr)) return SKY_E_INVALID;
+    if (n > ctx->max_chunks) return SKY_E_CAPACITY;
+    if (reinterpret_cast<uintptr_t>(d_src) & 15) return SKY_E_INVALID;
+    for (uint32_t i = 0; i < n; i++) {
+        if (src_off[i] & 15) return SKY_E_INVALID;
+        if (src_len[i] && !d_src) return SKY_E_INVALID;
+        if (frame_cap && frame_cap[i] < frame_need(src_len[i], flags)) return SKY_E_CAPACITY;
+    }
+    CK(ctx, cudaSetDevice(ctx->device));
+    Slot &s = ctx->slots[0];
+    if (s.ticket.busy) return SKY_E_BUSY;
+    cudaStream_t st = stream ? (cudaStream_t)stream : s.stream;
+    BatchMeta &m = s.meta;
+    uint32_t rows;
+    int rc = batch_geometry(n, src_len, rows, [&](uint32_t i, uint32_t nblk) {
+        m.h_desc[i] = ChunkDesc{(const uint8_t *)d_src + src_off[i], (uint8_t *)d_frames + frame_off[i], src_len[i], nblk};
+    });
+    if (rc != SKY_OK) return rc;
+    CK(ctx, cudaStreamSynchronize(st));  // (slot 0's metadata is free: nothing earlier on this stream still reads it)
+    memcpy(m.outlen.h, frame_len, n * sizeof(uint64_t));
+    CK(ctx, cudaMemcpyAsync(m.d_desc, m.h_desc, n * sizeof(ChunkDesc), cudaMemcpyHostToDevice, st));
+    if (content_xxh) CK(ctx, cudaMemcpyAsync(m.xxh, content_xxh, n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaEventRecord(s.ev_k0, st));
+    rc = launch_verify(ctx, s, st, n, rows, flags, frame_cap != nullptr);
+    if (rc != SKY_OK) return rc;
+    CK(ctx, cudaEventRecord(s.ev_k1, st));
+    CK(ctx, cudaStreamSynchronize(st));
+    if (status) memcpy(status, s.verify.status.h, n * sizeof(int32_t));
+    memcpy(frame_len, m.outlen.h, n * sizeof(uint64_t));
+    if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, s.ev_k0, s.ev_k1));
     return SKY_OK;
 }
 

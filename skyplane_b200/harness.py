@@ -35,6 +35,8 @@ def _drain_status(store: ChunkStore, acc: Dict):
                 acc["states"][rec["state"]] = acc["states"].get(rec["state"], 0) + 1
                 acc["comp"] += rec.get("compressed_size_bytes", 0)
                 acc["raw"] += rec.get("uncompressed_size_bytes", 0)
+                if "frame_verify_status" in rec:
+                    acc["verify"][rec["chunk_id"]] = rec["frame_verify_status"]
     except queue.Empty:
         pass
 
@@ -59,14 +61,16 @@ def run_stream(
     content_checksum: bool = False,
     compression_level: Optional[int] = None,
     block_checksum: bool = False,
+    verify_frames: bool = False,
 ) -> Dict:
     """Stream ``n_requests`` chunk requests (recycling ``pool_files`` by hard link) through the operator.
 
     The first ``warmup_requests`` completions are not timed (worker start-up: CUDA context, pinned staging).
-    ``high_ratio``, ``content_checksum``, ``compression_level`` and ``block_checksum`` are handed to the operator
-    (GatewayCompressHash's high-ratio frames, frames with LZ4's content checksum, the high-ratio level, frames with LZ4's
-    block checksums) when set.
-    Returns {"wall_s", "bytes", "records": [{chunk_id, pool_index, md5, raw_len, frame_path}], "status": {...}}.
+    ``high_ratio``, ``content_checksum``, ``compression_level``, ``block_checksum`` and ``verify_frames`` are handed to the
+    operator (GatewayCompressHash's high-ratio frames, frames with LZ4's content checksum, the high-ratio level, frames with
+    LZ4's block checksums, the GPU's check of every frame) when set.
+    Returns {"wall_s", "bytes", "records": [{chunk_id, pool_index, md5, raw_len, frame_path}], "status": {...},
+    "frame_verify": {chunk_id: status of every chunk whose frame failed the check}}.
     """
     chunk_dir = Path(chunk_dir)
     store = ChunkStore(chunk_dir)
@@ -80,10 +84,11 @@ def run_stream(
         **({"content_checksum": True} if content_checksum else {}),
         **({"compression_level": compression_level} if compression_level is not None else {}),
         **({"block_checksum": True} if block_checksum else {}),
+        **({"verify_frames": True} if verify_frames else {}),
     )
     op.start_workers()
     records: List[Dict] = []
-    status_acc = {"states": {}, "comp": 0, "raw": 0}
+    status_acc = {"states": {}, "comp": 0, "raw": 0, "verify": {}}
     pool_of: Dict[str, int] = {}
     sent = done = 0
     total_bytes = 0
@@ -153,7 +158,8 @@ def run_stream(
         time.sleep(0.01)
     store.chunk_status_queue.cancel_join_thread()
     status, comp, raw = status_acc["states"], status_acc["comp"], status_acc["raw"]
-    return {"wall_s": wall, "bytes": total_bytes, "records": records, "status": status, "compressed_bytes": comp, "uncompressed_bytes": raw}
+    return {"wall_s": wall, "bytes": total_bytes, "records": records, "status": status, "compressed_bytes": comp, "uncompressed_bytes": raw,
+            "frame_verify": status_acc["verify"]}
 
 
 def main():

@@ -15,6 +15,7 @@ LIB_PATH = _PKG / "libskychunk.so"
 SKY_OK = 0
 SKY_E_INVALID, SKY_E_NOGPU, SKY_E_CUDA, SKY_E_CAPACITY, SKY_E_BUSY, SKY_E_TICKET, SKY_E_NOMEM, SKY_E_NOKEY = -1, -2, -3, -4, -5, -6, -7, -8
 F_LZ4, F_MD5, F_E2EE, F_HC, F_CHECKSUM, F_BLOCK_CHECKSUM = 1, 2, 16, 32, 64, 128
+F_VERIFY = 1 << 12  # every frame is checked against its chunk on the GPU; one that fails is sent as its stored-block frame
 CHECKSUM_BYTES = 4  # F_CHECKSUM: the content checksum (u32le XXH32) behind the EndMark; F_BLOCK_CHECKSUM: as many per block
 BLOCK_BYTES = 65536
 # SKY_F_HC_LEVEL(l): the high-ratio level l (3..9: 2**(l - 1) chain candidates per position) in bits 8..11 of the flags;
@@ -25,14 +26,17 @@ HC_MIN_LEVEL, HC_DEFAULT_LEVEL, HC_MAX_LEVEL = 3, 5, 9
 BOX_OVERHEAD = 40
 # sky_decode status codes
 D_OK, D_BAD_HEADER, D_CORRUPT, D_SIZE, D_UNSUPPORTED, D_LAYOUT, D_TRUNCATED, D_AUTH, D_CHECKSUM = 0, -1, -2, -3, -4, -5, -6, -7, -8
+D_MISMATCH = -9  # F_VERIFY: the frame is well formed but decodes to other bytes than its chunk
 D_NAMES = {0: "ok", -1: "bad frame header", -2: "corrupt block", -3: "size mismatch", -4: "unsupported frame feature",
-           -5: "unexpected block layout", -6: "truncated frame", -7: "box authentication failed", -8: "checksum mismatch"}
+           -5: "unexpected block layout", -6: "truncated frame", -7: "box authentication failed", -8: "checksum mismatch",
+           -9: "frame decodes to other bytes"}
 
 # every symbol include/skychunk.h declares (tests check the .so exports exactly these)
 ABI_SYMBOLS = (
     "sky_strerror", "sky_last_error", "sky_abi_version", "sky_device_count", "sky_device_pci_bus_id", "sky_kernel_config", "sky_frame_bound",
     "sky_ctx_create", "sky_ctx_destroy", "sky_pinned_alloc", "sky_pinned_free",
-    "sky_submit", "sky_wait", "sky_set_e2ee_key", "sky_box_bound", "sky_process_device", "sky_decode_device", "sky_decode",
+    "sky_submit", "sky_wait", "sky_wait_verify", "sky_set_e2ee_key", "sky_box_bound", "sky_process_device", "sky_verify_device",
+    "sky_decode_device", "sky_decode",
     "sky_device_alloc", "sky_device_free", "sky_memcpy_h2d", "sky_memcpy_d2h", "sky_launch_count",
 )
 
@@ -104,11 +108,16 @@ def lib() -> ctypes.CDLL:
     L.sky_box_bound.restype = u64
     L.sky_wait.argtypes = [vp, u64, p_u64, vp, ctypes.POINTER(ctypes.c_float)]
     L.sky_wait.restype = i32
+    L.sky_wait_verify.argtypes = [vp, u64, p_u64, vp, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_float)]
+    L.sky_wait_verify.restype = i32
     L.sky_process_device.argtypes = [vp, u32, vp, p_u64, p_u64, vp, p_u64, p_u64, u32, vp, p_u64, vp, ctypes.POINTER(ctypes.c_float)]
     L.sky_process_device.restype = i32
     p_i32 = ctypes.POINTER(ctypes.c_int32)
     L.sky_decode_device.argtypes = [vp, u32, vp, p_u64, p_u64, vp, p_u64, p_u64, vp, p_i32, vp, ctypes.POINTER(ctypes.c_float)]
     L.sky_decode_device.restype = i32
+    L.sky_verify_device.argtypes = [vp, u32, vp, p_u64, p_u64, vp, p_u64, p_u64, p_u64, ctypes.POINTER(ctypes.c_uint32), u32, vp, p_i32,
+                                    ctypes.POINTER(ctypes.c_float)]
+    L.sky_verify_device.restype = i32
     L.sky_decode.argtypes = [vp, u32, ctypes.POINTER(vp), p_u64, ctypes.POINTER(vp), p_u64, u32, p_i32, vp, ctypes.POINTER(ctypes.c_float)]
     L.sky_decode.restype = i32
     L.sky_device_alloc.argtypes = [vp, u64, ctypes.POINTER(vp)]
@@ -295,6 +304,19 @@ class Context:
         raw = bytes(md5)
         return list(out), [raw[16 * i : 16 * i + 16] for i in range(n)], ms.value
 
+    def wait_verify(self, ticket: int):
+        """wait() for a ticket submitted with F_VERIFY -> (out_lens, digests, verify, kernel_ms); verify[i] is 0 or the D_*
+        code of chunk i's frame as the compressor made it (its payload is then the stored-block frame)."""
+        n, _keep = self._inflight[ticket]
+        out = (ctypes.c_uint64 * n)()
+        md5 = (ctypes.c_ubyte * (16 * n))()
+        ver = (ctypes.c_int32 * n)()
+        ms = ctypes.c_float(0)
+        self._check(lib().sky_wait_verify(self._h, ticket, out, md5, ver, ctypes.byref(ms)))
+        del self._inflight[ticket]
+        raw = bytes(md5)
+        return list(out), [raw[16 * i : 16 * i + 16] for i in range(n)], list(ver), ms.value
+
     # ------------------------------------------------------------------ device-resident path
     def process_device(self, d_src: int, src_off: Sequence[int], src_len: Sequence[int], d_dst: int, dst_off: Sequence[int],
                        dst_cap: Sequence[int], flags: int = 0, stream: int = 0):
@@ -310,6 +332,23 @@ class Context:
         )
         raw = bytes(md5)
         return list(out), [raw[16 * i : 16 * i + 16] for i in range(n)], ms.value
+
+    def verify_device(self, d_src: int, src_off: Sequence[int], src_len: Sequence[int], d_frames: int, frame_off: Sequence[int],
+                      frame_len: Sequence[int], frame_cap: Optional[Sequence[int]] = None, content_xxh: Optional[Sequence[int]] = None,
+                      flags: int = 0, stream: int = 0):
+        """F_VERIFY's check of frames already in HBM against their chunks (sky_verify_device).  flags: the frame flags they
+        were made with; content_xxh: the chunks' XXH32, exactly when flags has F_CHECKSUM.  frame_cap None: check only;
+        otherwise failing frames are rewritten as stored-block frames.  -> (status, frame_len, kernel_ms)."""
+        n = len(src_len)
+        U = ctypes.c_uint64 * n
+        fl = U(*frame_len)
+        st = (ctypes.c_int32 * n)()
+        ms = ctypes.c_float(0)
+        self._check(lib().sky_verify_device(self._h, n, d_src, U(*src_off), U(*src_len), d_frames, U(*frame_off), fl,
+                                            U(*frame_cap) if frame_cap is not None else None,
+                                            (ctypes.c_uint32 * n)(*content_xxh) if content_xxh is not None else None, flags,
+                                            stream or None, st, ctypes.byref(ms)))
+        return list(st), list(fl), ms.value
 
     # ------------------------------------------------------------------ receiver side
     def decode_device(self, d_frames: int, frame_off: Sequence[int], frame_len: Sequence[int], d_out: int, out_off: Sequence[int],

@@ -20,6 +20,7 @@ and error conventions.  CUDA is initialised lazily inside the worker process, ne
 """
 from __future__ import annotations
 
+import logging
 import os
 import queue
 import time
@@ -31,6 +32,8 @@ from typing import List, Optional
 from skyplane_b200.chunk import ChunkRequest, ChunkState
 from skyplane_b200.chunk_store import ChunkStore
 from skyplane_b200.gateway_queue import GatewayQueue
+
+logger = logging.getLogger(__name__)
 
 
 class GatewayOperator(ABC):
@@ -137,6 +140,7 @@ class GatewayCompressHash(GatewayOperator):
         content_checksum: bool = False,
         compression_level: Optional[int] = None,
         block_checksum: bool = False,
+        verify_frames: bool = False,
     ):
         """use_compression / e2ee_key_bytes: GatewaySender's arguments of the same name (gateway_operator.py:154-168):
         ``use_compression=False`` digests the chunk and lets it pass through uncompressed (``is_compressed=False``);
@@ -151,6 +155,9 @@ class GatewayCompressHash(GatewayOperator):
         time), 0..2 with the fast compressor; ``high_ratio`` alone means level 5.  Needs ``use_compression``.
         block_checksum: every block of the frame carries LZ4's block checksum (XXH32 of the block as stored, python-lz4's
         argument of the same name), so any LZ4 decoder rejects a damaged block before decoding it.  Needs ``use_compression``.
+        verify_frames: the GPU checks every frame against its chunk before it leaves (``ChunkStage.launch(verify=True)``); a
+        frame that would not restore the chunk is sent as the chunk's stored-block frame instead, a warning names the chunk
+        and the failed check, and the chunk's ``complete`` record carries ``frame_verify_status``.  Needs ``use_compression``.
         sink: ``callable(worker_id) -> socket``, called once in each worker.  With a sink the worker sends every payload
         straight from the pinned staging slot (``wire.send_results``: WireProtocolHeader + payload, no intermediate bytes
         object, no frame file) -- the tail of ``GatewaySender.process`` (gateway_operator.py:367-402)."""
@@ -165,6 +172,9 @@ class GatewayCompressHash(GatewayOperator):
         if block_checksum and not self.use_compression:
             raise ValueError("block_checksum is carried by the LZ4 frame: it needs use_compression")
         self.block_checksum = bool(block_checksum)
+        if verify_frames and not self.use_compression:
+            raise ValueError("verify_frames checks the LZ4 frames: it needs use_compression")
+        self.verify_frames = bool(verify_frames)
         from skyplane_b200 import native
 
         native.hc_flags(compression_level, self.high_ratio, self.use_compression)  # (ValueError on a bad level, here and not in a worker)
@@ -318,6 +328,8 @@ class GatewayCompressHash(GatewayOperator):
             opts["level"] = self.compression_level
         if self.block_checksum:
             opts["block_checksum"] = True
+        if self.verify_frames:
+            opts["verify"] = True
         stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None, **opts)
         return True
 
@@ -339,6 +351,13 @@ class GatewayCompressHash(GatewayOperator):
         for r, res in zip(reqs, results):
             r.chunk.md5_hash = res.md5
             r._stage_meta = {"compressed_size_bytes": res.comp_len, "uncompressed_size_bytes": res.raw_len}
+            if res.verify_status:
+                from skyplane_b200 import native
+
+                logger.warning("[%s:%s] chunk %s: its LZ4 frame failed the GPU check (%d, %s); sending its stored-block frame",
+                               self.handle, self.worker_id, r.chunk.chunk_id, res.verify_status,
+                               native.D_NAMES.get(res.verify_status, "?"))
+                r._stage_meta["frame_verify_status"] = res.verify_status
         if self.sink is not None:
             from skyplane_b200 import wire
 

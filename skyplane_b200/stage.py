@@ -30,6 +30,8 @@ class StageResult:
     comp_len: int  # WireProtocolHeader.data_len (length of `frame`)
     is_compressed: bool = True  # WireProtocolHeader.is_compressed
     is_encrypted: bool = False
+    verify_status: int = 0  # launch(verify=True): 0, or the native.D_* code of the frame as compressed (`frame` is then the
+    #                         chunk's stored-block frame)
 
     def frame_bytes(self) -> bytes:
         return bytes(self.frame)
@@ -162,7 +164,7 @@ class ChunkStage:
         self._has_key = key is not None
 
     def launch(self, slot: _Slot, compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None, hc: bool = False,
-               checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False) -> _Slot:
+               checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False, verify: bool = False) -> _Slot:
         """compress=False is the reference's `compress: false` (digest only, the chunk passes through);
         encrypt=True seals every payload with the stage's key (nonces: 24 bytes per chunk, default os.urandom);
         hc=True makes the frames with the high-ratio parse (F_HC): same frame format, fewer bytes, more GPU time;
@@ -170,7 +172,10 @@ class ChunkStage:
         block_checksum=True gives every block of the frame LZ4's block checksum (F_BLOCK_CHECKSUM), which any LZ4 decoder
         verifies before it decodes the block;
         level is python-lz4's compression_level: 3..9 runs the high-ratio parse at that level (2**(level - 1) chain
-        candidates per position: more ratio for more GPU time), hc=True alone means level 5, 0..2 is the fast path."""
+        candidates per position: more ratio for more GPU time), hc=True alone means level 5, 0..2 is the fast path;
+        verify=True checks every frame against its chunk on the GPU before it is sealed or copied out (F_VERIFY): a frame
+        that would not restore the chunk is replaced by the chunk's stored-block frame and its StageResult.verify_status
+        says why."""
         if not slot.lens:
             raise ValueError("empty batch")
         if hc and not compress:
@@ -179,6 +184,8 @@ class ChunkStage:
             raise ValueError("checksum=True is carried by the LZ4 frame: it needs compress=True")
         if block_checksum and not compress:
             raise ValueError("block_checksum=True is carried by the LZ4 frame: it needs compress=True")
+        if verify and not compress:
+            raise ValueError("verify=True checks the LZ4 frames: it needs compress=True")
         hc_bits = native.hc_flags(level, hc, compress)
         if hc_bits and not native.kernel_config()["hc_depth"]:
             raise native.SkyChunkError(native.SKY_E_INVALID, f"{native.LIB_PATH.name} was built without the high-ratio kernel (F_HC)")
@@ -187,7 +194,8 @@ class ChunkStage:
         base_in, base_out = slot.inp.addr, slot.out.addr
         src = [base_in + o for o in slot.in_off]
         flags = (native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0) | hc_bits
-                 | (native.F_CHECKSUM if checksum else 0) | (native.F_BLOCK_CHECKSUM if block_checksum else 0))
+                 | (native.F_CHECKSUM if checksum else 0) | (native.F_BLOCK_CHECKSUM if block_checksum else 0)
+                 | (native.F_VERIFY if verify else 0))
         if encrypt and nonces is None:
             nonces = os.urandom(24 * len(slot.lens))  # what nacl.utils.random(24) draws per message
         if compress or encrypt:
@@ -201,24 +209,32 @@ class ChunkStage:
         return slot
 
     def collect(self, slot: _Slot) -> List[StageResult]:
-        out_lens, digests, self.last_kernel_ms = self.ctx.wait(slot.ticket)
+        if slot.flags & native.F_VERIFY:
+            out_lens, digests, verify, self.last_kernel_ms = self.ctx.wait_verify(slot.ticket)
+        else:
+            out_lens, digests, self.last_kernel_ms = self.ctx.wait(slot.ticket)
+            verify = [0] * len(slot.lens)
         comp, enc = bool(slot.flags & native.F_LZ4), bool(slot.flags & native.F_E2EE)
         res = []
-        for io, o, cl, dg, n in zip(slot.in_off, slot.out_off, out_lens, digests, slot.lens):
+        for io, o, cl, dg, n, v in zip(slot.in_off, slot.out_off, out_lens, digests, slot.lens, verify):
             payload = slot.out.view[o : o + cl] if (comp or enc) else slot.inp.view[io : io + n]
-            res.append(StageResult(frame=payload, md5=dg, raw_len=n, comp_len=len(payload), is_compressed=comp, is_encrypted=enc))
+            res.append(StageResult(frame=payload, md5=dg, raw_len=n, comp_len=len(payload), is_compressed=comp, is_encrypted=enc,
+                                   verify_status=v))
         slot.ticket = None
         self._free.append(slot)
         return res
 
     # ------------------------------------------------------------------ sync convenience
     def process(self, chunks: Sequence[BytesLike], compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None,
-                hc: bool = False, checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False) -> List[StageResult]:
+                hc: bool = False, checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False,
+                verify: bool = False) -> List[StageResult]:
         """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes (hc, checksum,
-        level, block_checksum: see launch)."""
+        level, block_checksum, verify: see launch)."""
         native.hc_flags(level, hc, compress)  # (bad arguments fail before the first batch)
         if block_checksum and not compress:
             raise ValueError("block_checksum=True is carried by the LZ4 frame: it needs compress=True")
+        if verify and not compress:
+            raise ValueError("verify=True checks the LZ4 frames: it needs compress=True")
         out: List[StageResult] = []
         i = 0
         while i < len(chunks):
@@ -230,10 +246,11 @@ class ChunkStage:
             if j == i:
                 self.release(slot)
                 raise native.SkyChunkError(native.SKY_E_CAPACITY, f"chunk of {memoryview(chunks[i]).nbytes} bytes exceeds max_batch_bytes")
-            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum, level, block_checksum)
+            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum, level, block_checksum,
+                        verify)
             for r in self.collect(slot):
                 out.append(StageResult(frame=memoryview(bytes(r.frame)), md5=r.md5, raw_len=r.raw_len, comp_len=r.comp_len,
-                                       is_compressed=r.is_compressed, is_encrypted=r.is_encrypted))
+                                       is_compressed=r.is_compressed, is_encrypted=r.is_encrypted, verify_status=r.verify_status))
             i = j
         return out
 

@@ -9,7 +9,9 @@ hc9-block-checksum (SKY_F_BLOCK_CHECKSUM: the same frames with LZ4's block check
 --decode-from liblz4[-linked][-checksums] times the receiver on liblz4's level-0 frames made on the host from the same
 input: independent or linked blocks, without checksums or with block and content checksums.
 --ref-ratio adds the reference's ratio (liblz4 level 0, linked blocks) on the distinct chunks; --liblz4-level9 times liblz4
-level 9 with independent blocks on all of the host's cores (the rate the reference's sender would get from that level)."""
+level 9 with independent blocks on all of the host's cores (the rate the reference's sender would get from that level).
+--verify also times SKY_F_VERIFY's check (sky_verify_device, check only) of every frame set right after it is made, in the
+same iterations: kernel_ms (frames), verify_ms (their check) and kernel_plus_verify_ms; every status must be 0."""
 import argparse
 import json
 import multiprocessing as mp
@@ -108,6 +110,7 @@ def main():
                     "(frames made on the host by liblz4: linked blocks, block and content checksums)")
     ap.add_argument("--ref-ratio", action="store_true", help="also the reference's ratio on the distinct chunks (CPU)")
     ap.add_argument("--liblz4-level9", action="store_true", help="also liblz4 level 9 on all host cores (CPU)")
+    ap.add_argument("--verify", action="store_true", help="also time the frame check (SKY_F_VERIFY) of each flag set's frames")
     a = ap.parse_args()
     dev = torch.device("cuda", 0)
     FL = {"lz4": native.F_LZ4, "md5": native.F_MD5, "both": 0, "hc": native.F_HC, "hc-lz4": native.F_HC | native.F_LZ4,
@@ -142,16 +145,30 @@ def main():
             src_off = [i * stride for i in range(n)]
             dst_off = [i * so for i in range(n)]
             for fl in a.flags.split(","):
-                ms = []
+                ms, vms, vok = [], [], True
                 for it in range(a.iters + 1):
                     torch.cuda.synchronize()
                     out_lens, dg, kms = ctx.process_device(d_in.data_ptr(), src_off, [chunk_bytes] * n, d_out.data_ptr(), dst_off, [bound] * n, FL[fl], 0)
+                    if a.verify:  # the check of the frames just made, alternating with their making
+                        xxh = None
+                        if FL[fl] & native.F_CHECKSUM:  # the content checksums the frames carry, from behind their EndMarks
+                            tail = [d_out[o + l - 4 : o + l].cpu().numpy().tobytes() for o, l in zip(dst_off, out_lens)]
+                            xxh = [int.from_bytes(t, "little") for t in tail]
+                        st, _, v = ctx.verify_device(d_in.data_ptr(), src_off, [chunk_bytes] * n, d_out.data_ptr(), dst_off, out_lens,
+                                                     None, xxh, FL[fl] or native.F_LZ4, 0)
+                        vok = vok and all(x == 0 for x in st)
+                        if it:
+                            vms.append(v)
                     if it:
                         ms.append(kms)
                 k = statistics.median(ms)
                 tot = n * chunk_bytes
-                print(json.dumps({"workload": wl, "chunk_mib": float(sz), "chunks": n, "flags": fl, "kernel_ms": k, "raw_input_gbs": tot / k / 1e6,
-                                  "ratio": (tot / sum(out_lens)) if sum(out_lens) else None, "per_stream_gbs": chunk_bytes / k / 1e6}), flush=True)
+                row = {"workload": wl, "chunk_mib": float(sz), "chunks": n, "flags": fl, "kernel_ms": k, "raw_input_gbs": tot / k / 1e6,
+                       "ratio": (tot / sum(out_lens)) if sum(out_lens) else None, "per_stream_gbs": chunk_bytes / k / 1e6}
+                if a.verify:
+                    v = statistics.median(vms)
+                    row.update({"verify_ms": v, "kernel_plus_verify_ms": k + v, "verify_raw_gbs": tot / v / 1e6, "verify_all_ok": vok})
+                print(json.dumps(row), flush=True)
             if a.decode:
                 # receiver side: decode the frames just produced (d_out) back into a fresh buffer + MD5 of the result
                 if a.decode_from.startswith("liblz4"):
