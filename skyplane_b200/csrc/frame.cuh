@@ -1,16 +1,52 @@
 // frame.cuh -- the sender's batch and frame contract, shared by both block compressors (sky_fused_kernel in skychunk.cu,
-// sky_hc_kernel in lz4hc.cuh): the batch descriptors, the block claim, the block load into shared memory, the block's
-// placement in its frame through the OFF chain, and the per-warp write-out.
+// sky_hc_kernel in lz4hc.cuh) and the frame check's repair: the batch descriptors, the final frame header (the one place
+// that maps the batch's flags to FLG bits), the block claim, the block load into shared memory, the block's placement in
+// its frame through the OFF chain, the per-warp write-out, and the block and content checksums.
 //
 // OFF chain (one word per chunk): OFF = (next block index << 40) | frame offset of that block, a prefix sum handed from
 // block j-1 to block j as soon as j-1 knows its compressed size -- before it has written a byte, so offsets race down the
 // chain.  The host starts every chunk's word at (0 << 40) | kFrameHeaderBytes.  Waiting is deadlock-free: a CTA only waits
 // on lower-numbered work items, all of which were claimed earlier by running CTAs.
 #pragma once
+#include "../../include/skychunk.h"
 #include "lz4.cuh"
 #include "xxh32.cuh"
 
 namespace sky {
+
+constexpr uint32_t kFrameHeaderBytes = 15;  // frame header with content size: magic, FLG, BD, 8-byte content size, header checksum
+
+// Frame header bytes of an n-byte chunk: the content size is omitted for an empty chunk (0 means "unknown" to LZ4F).
+__device__ __forceinline__ uint32_t frame_header_bytes(uint64_t n) { return n ? kFrameHeaderBytes : 7u; }
+
+// The FLG bits a batch's flags set: C.Checksum (0x04) with SKY_F_CHECKSUM, B.Checksum (0x10) with SKY_F_BLOCK_CHECKSUM.
+__device__ __forceinline__ uint32_t frame_flg(uint32_t flags) {
+    return ((flags & SKY_F_CHECKSUM) ? 0x04u : 0u) | ((flags & SKY_F_BLOCK_CHECKSUM) ? 0x10u : 0u);
+}
+
+__device__ __forceinline__ void st_u32le(uint8_t *p, uint32_t v) {
+    p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24);
+}
+
+// Single thread: writes the final frame header of an n-byte chunk made with the batch's `flags`; returns its size.
+__device__ __forceinline__ uint32_t write_frame_header(uint8_t *dst, uint64_t n, uint32_t flags) {
+    uint8_t d[10];
+    d[1] = 0x40;  // BD: 64 KiB blocks
+    st_u32le(dst, 0x184D2204u);  // magic
+    if (n == 0) {
+        d[0] = (uint8_t)(0x60u | frame_flg(flags));  // v01 | B.Indep
+        dst[4] = d[0]; dst[5] = d[1];
+        dst[6] = (uint8_t)(xxh32_small(d, 2) >> 8);
+        return 7;
+    }
+    d[0] = (uint8_t)(0x68u | frame_flg(flags));  // v01 | B.Indep | C.Size
+#pragma unroll
+    for (int i = 0; i < 8; i++) d[2 + i] = (uint8_t)(n >> (8 * i));
+#pragma unroll
+    for (int i = 0; i < 10; i++) dst[4 + i] = d[i];
+    dst[kFrameHeaderBytes - 1] = (uint8_t)(xxh32_small(d, 10) >> 8);
+    return kFrameHeaderBytes;
+}
 
 constexpr uint32_t kInBytes = kBlock + 128;  // a block buffer in shared memory, + slack: unaligned 4-byte reads may touch the word after the last byte
 constexpr uint32_t kLoadPiece = 8192;        // bytes per bulk copy of the block load
@@ -70,8 +106,12 @@ __device__ __forceinline__ void st_release32(uint32_t *p, uint32_t v) {
 }
 
 // One thread: claim the next block that has LZ4 work (empty chunks are finished on the spot) and describe it to the CTA.
+// Block 0's claim writes the frame header.
 __device__ __forceinline__ void claim_block(const Params &p, BlockDesc *d) {
     const uint32_t total = p.rows * p.n_chunks;
+    // read per claim: hoisted out of the kernel's block loop, the FLG bits would hold a register there (sky_fused_kernel spills)
+    uint32_t flags = p.flags;
+    asm volatile("" : "+r"(flags));
     for (;;) {
         const uint32_t w = atomicAdd(p.counters, 1u);
         if (w >= total) {
@@ -82,8 +122,8 @@ __device__ __forceinline__ void claim_block(const Params &p, BlockDesc *d) {
         const ChunkDesc cd = p.chunks[c];
         if (cd.nblk == 0) {
             if (j == 0) {  // empty chunk: 7-byte header + EndMark
-                const uint32_t h = write_frame_header(cd.dst, 0);
-                cd.dst[h] = cd.dst[h + 1] = cd.dst[h + 2] = cd.dst[h + 3] = 0;
+                const uint32_t h = write_frame_header(cd.dst, 0, flags);
+                st_u32le(cd.dst + h, 0);
                 p.out_len[c] = h + 4;
             }
             continue;
@@ -97,7 +137,7 @@ __device__ __forceinline__ void claim_block(const Params &p, BlockDesc *d) {
         d->L = (uint32_t)min((uint64_t)kBlock, cd.len - boff);
         d->last = (j + 1 == cd.nblk);
         d->valid = 1;
-        if (j == 0) write_frame_header(cd.dst, cd.len);
+        if (j == 0) write_frame_header(cd.dst, cd.len, flags);
         return;
     }
 }
@@ -132,12 +172,9 @@ __device__ __forceinline__ BlockPlace place_block(const Params &p, const BlockDe
     const uint64_t off = st & kOffMask;
     const uint64_t end = off + 4 + (raw ? L : csize) + (kBlkChk ? 4 : 0);
     if (!d.last) st_release(cw, ((uint64_t)(d.j + 1) << kOffBits) | end);
-    uint8_t *hdr = d.dst + off;
-    const uint32_t hword = raw ? (L | 0x80000000u) : csize;
-    hdr[0] = (uint8_t)hword; hdr[1] = (uint8_t)(hword >> 8); hdr[2] = (uint8_t)(hword >> 16); hdr[3] = (uint8_t)(hword >> 24);
+    st_u32le(d.dst + off, raw ? (L | 0x80000000u) : csize);
     if (d.last) {
-        uint8_t *e = d.dst + end;
-        e[0] = e[1] = e[2] = e[3] = 0;  // EndMark
+        st_u32le(d.dst + end, 0);  // EndMark
         p.out_len[d.c] = end + 4;
     }
     return BlockPlace{off + 4, raw};
@@ -157,7 +194,7 @@ __device__ __forceinline__ void copy_block(uint8_t *out, const uint8_t *src, uin
 // the data.  place_block<true> has passed the next offset on before any of this, so the hash is never on the OFF chain.
 __device__ __forceinline__ void block_checksum(const uint8_t *src, uint32_t n, uint8_t *at, unsigned lane) {
     const uint32_t x = xxh32_warp(src, n, lane);
-    if (lane == 0) { at[0] = (uint8_t)x; at[1] = (uint8_t)(x >> 8); at[2] = (uint8_t)(x >> 16); at[3] = (uint8_t)(x >> 24); }
+    if (lane == 0) st_u32le(at, x);
 }
 // A block whose checksum is hashed later from its bytes in the frame, by one warp of the CTA that wrote them, after a CTA
 // barrier has ordered those writes before its reads: the warp runs it where it would otherwise wait, off the CTA's next
@@ -184,23 +221,12 @@ __device__ __forceinline__ void set_pending(PendingChecksum *pc, uint8_t *data, 
     }
 }
 
-// Frame-descriptor epilogue of chunk c's finished frame, one thread: FLG gains `flg` (SKY_F_CHECKSUM: C.Checksum 0x04,
-// SKY_F_BLOCK_CHECKSUM: B.Checksum 0x10; 0x68 -> 0x6C / 0x78 / 0x7C, 0x60 -> 0x64 / 0x70 / 0x74 for an empty chunk) and
-// the header checksum byte follows.  With the content checksum (xxh != null) xxh[c], the XXH32 of the chunk, goes behind
-// the EndMark at out_len[c], which grows by 4.
-__device__ __forceinline__ void finish_frame(const ChunkDesc *chunks, const uint32_t *xxh, uint64_t *out_len, uint32_t c, uint32_t flg) {
-    const ChunkDesc cd = chunks[c];
-    uint8_t *f = cd.dst;
-    const uint32_t dlen = cd.len ? 10u : 2u;  // FLG, BD (+ content size)
-    f[4] |= (uint8_t)flg;
-    uint8_t d[10];
-    for (uint32_t i = 0; i < dlen; i++) d[i] = f[4 + i];
-    f[4 + dlen] = (uint8_t)(xxh32_small(d, dlen) >> 8);
-    if (!xxh) return;
-    const uint64_t end = out_len[c];
-    const uint32_t x = xxh[c];
-    f[end] = (uint8_t)x; f[end + 1] = (uint8_t)(x >> 8); f[end + 2] = (uint8_t)(x >> 16); f[end + 3] = (uint8_t)(x >> 24);
-    out_len[c] = end + 4;
+// SKY_F_CHECKSUM, one thread, on a finished frame of *len bytes (its header already carries C.Checksum): the content
+// checksum `xxh`, the XXH32 of the chunk, goes behind the EndMark and *len grows by 4.
+__device__ __forceinline__ void finish_frame(uint8_t *frame, uint64_t *len, uint32_t xxh) {
+    const uint64_t end = *len;
+    st_u32le(frame + end, xxh);
+    *len = end + 4;
 }
 
 }  // namespace sky

@@ -146,29 +146,6 @@ __device__ __forceinline__ uint32_t xxh32_small(const uint8_t *p, uint32_t len) 
     return h;
 }
 
-constexpr uint32_t kFrameHeaderBytes = 15;  // frame header with content size: magic, FLG, BD, 8-byte content size, header checksum
-
-// Writes the frame header for an n-byte chunk at dst; returns its size (kFrameHeaderBytes, or 7 when n == 0).
-// Single thread.
-__device__ __forceinline__ uint32_t write_frame_header(uint8_t *dst, uint64_t n) {
-    uint8_t d[10];
-    d[1] = 0x40;  // BD: 64 KiB blocks
-    dst[0] = 0x04; dst[1] = 0x22; dst[2] = 0x4D; dst[3] = 0x18;
-    if (n == 0) {
-        d[0] = 0x60;  // v01 | B.Indep ; content size omitted (0 means "unknown" to LZ4F)
-        dst[4] = d[0]; dst[5] = d[1];
-        dst[6] = (uint8_t)(xxh32_small(d, 2) >> 8);
-        return 7;
-    }
-    d[0] = 0x68;  // v01 | B.Indep | C.Size
-#pragma unroll
-    for (int i = 0; i < 8; i++) d[2 + i] = (uint8_t)(n >> (8 * i));
-#pragma unroll
-    for (int i = 0; i < 10; i++) dst[4 + i] = d[i];
-    dst[kFrameHeaderBytes - 1] = (uint8_t)(xxh32_small(d, 10) >> 8);
-    return kFrameHeaderBytes;
-}
-
 // ---- sequence emission ----------------------------------------------------------------------------
 // Emits token, literal-length bytes, literals, offset, match-length bytes.  All lanes call it with
 // warp-uniform arguments; returns the new output cursor.

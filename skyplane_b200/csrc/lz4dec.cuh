@@ -10,6 +10,7 @@
 //                 decode block j after block j-1 of the same chunk (matches may reach into earlier output).
 //                 A block checksum is verified before the block is decoded, as liblz4 does; the content checksum
 //                 by the MD5 lanes, which hash every decoded byte anyway (md5_warp<true>).
+// The sender's frame check (lz4verify.cuh) shares frame_index, the block claim, the block-status protocol and read_ext.
 // Every read and write is bounds-checked: a malformed frame yields an error status, never an out-of-range access.
 // The decoded size of block j is taken to be min(64 KiB, raw_len - j*64 KiB) -- true for liblz4 and for our
 // encoder (only the last block is short); anything else is reported as SKY_D_LAYOUT.
@@ -30,11 +31,31 @@ constexpr int32_t kDecLayout = -5;      // block structure does not match 64 KiB
 constexpr int32_t kDecTruncated = -6;   // frame ends inside a header, block, checksum or before the content checksum
 constexpr int32_t kDecChecksum = -8;    // a block checksum or the content checksum does not match (-7 is SKY_D_AUTH)
 
-// While blocks decode, a chunk's status may hold block_fail(j, code): below every code above, and ordered by block index
-// first, so atomicMin keeps the earliest failing block.  Once every block is done, the chunk's MD5 lane turns it back
-// into `code`.
+// Per-block status of sky_decode_kernel and sky_verify_kernel: while blocks run, a chunk's status may hold
+// block_fail(j, code): below every code above, and ordered by block index first, so atomicMin keeps the earliest failing
+// block.  Once every block is done, settle_status turns it back into `code`.
 constexpr int32_t kBlockFail = INT32_MIN;
 __device__ __forceinline__ int32_t block_fail(uint32_t j, int32_t code) { return kBlockFail + (int32_t)(j * 16u) - code; }
+__device__ __forceinline__ int32_t settle_status(int32_t s) { return s < kDecChecksum ? -((s - kBlockFail) & 15) : s; }
+
+// Block j still runs unless the frame or an earlier block failed; a content checksum failure (kDecChecksum) yields to
+// any block failure.  The decoder's MD5 lane sets kDecChecksum only once every row of the chunk has passed its gate, i.e.
+// after every decode warp of the chunk has read the status, so the one rule serves both kernels.
+__device__ __forceinline__ bool block_may_run(int32_t st, uint32_t j) {
+    return st == kDecOk || st == kDecChecksum || (st < kDecChecksum && st > block_fail(j, 0));
+}
+
+// Whole warp: claim work item w = j * n_chunks + c (block row j of every chunk, then row j + 1); false once all are taken.
+__device__ __forceinline__ bool claim_row_major(uint32_t *counter, uint32_t n_chunks, uint32_t rows, unsigned lane, uint32_t &c,
+                                                uint32_t &j) {
+    uint32_t w = 0;
+    if (lane == 0) w = atomicAdd(counter, 1u);
+    w = __shfl_sync(kFull, w, 0);
+    if (w >= rows * n_chunks) return false;
+    c = w % n_chunks;
+    j = w / n_chunks;
+    return true;
+}
 
 constexpr uint32_t kChkBlock = 1, kChkContent = 2;  // DecChunk::checks
 
@@ -137,6 +158,17 @@ __device__ __forceinline__ void warp_match_copy(uint8_t *op, uint32_t offset, ui
     }
 }
 
+// Length extension of a 4-bit field that reads 15; false when it runs off the block's bytes.
+__device__ __forceinline__ bool read_ext(const uint8_t *blk, uint32_t slen, uint32_t &ip, uint32_t &len) {
+    uint32_t s;
+    do {
+        if (ip >= slen) return false;
+        s = blk[ip++];
+        len += s;
+    } while (s == 255 && len < (1u << 24));
+    return true;
+}
+
 // One warp decodes one compressed block: src[0, slen) -> out[pos, pos + want); `low` = lowest output position a
 // match may reference.  Returns kDecOk or an error; all lanes return the same value.
 __device__ __forceinline__ int32_t lz4_decode_block(const uint8_t *src, uint32_t slen, uint8_t *out, uint64_t pos, uint32_t want,
@@ -149,14 +181,7 @@ __device__ __forceinline__ int32_t lz4_decode_block(const uint8_t *src, uint32_t
         if (ip >= slen) return kDecCorrupt;
         const uint32_t token = src[ip++];
         uint32_t ll = token >> 4;
-        if (ll == 15) {
-            uint32_t s;
-            do {
-                if (ip >= slen) return kDecCorrupt;
-                s = src[ip++];
-                ll += s;
-            } while (s == 255 && ll < (1u << 24));
-        }
+        if (ll == 15 && !read_ext(src, slen, ip, ll)) return kDecCorrupt;
         if (ll > slen - ip || op + ll > oend) return kDecCorrupt;
         warp_copy(out + op, src + ip, ll, lane);
         ip += ll;
@@ -167,14 +192,7 @@ __device__ __forceinline__ int32_t lz4_decode_block(const uint8_t *src, uint32_t
         ip += 2;
         if (offset == 0 || offset > op - low) return kDecCorrupt;
         uint32_t ml = token & 15;
-        if (ml == 15) {
-            uint32_t s;
-            do {
-                if (ip >= slen) return kDecCorrupt;
-                s = src[ip++];
-                ml += s;
-            } while (s == 255 && ml < (1u << 24));
-        }
+        if (ml == 15 && !read_ext(src, slen, ip, ml)) return kDecCorrupt;
         ml += kMinMatch;
         if (op + ml > oend) return kDecCorrupt;
         __syncwarp();  // the literals just written may be the match source

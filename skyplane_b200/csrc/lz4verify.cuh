@@ -2,17 +2,16 @@
 // LZ4 decoder?  Where one does not, the chunk's stored-block frame takes its place before anything is sealed or sent.
 //
 // Three launches on the batch's stream, after the frame epilogue (finish_frame) and before the seal:
-//   sky_verify_index_kernel  : one thread per chunk.  The header must be exactly the one the stage writes for the batch's
-//                              flags (FLG 0x68 / 0x6C / 0x78 / 0x7C, or 0x60 / 0x64 / 0x70 / 0x74 for an empty chunk, BD
-//                              0x40), then frame_index (lz4dec.cuh) checks magic, content size and HC byte and walks the
-//                              block words with nblk taken from the chunk's length; the EndMark must follow the last block,
-//                              the frame must end right behind it (and its content checksum), and the content checksum must
-//                              be the XXH32 the MD5 lanes computed from the chunk.
-//   sky_verify_kernel        : one warp per 64 KiB block, claimed row-major.  The block checksum over the block's stored
-//                              bytes, then a stored block's bytes against the chunk, or a compare-decode of a compressed
-//                              block against the chunk.
-//   sky_verify_settle_kernel : one CTA per chunk.  The chunk's status, and for a failing chunk with repair on, its frame
-//                              rewritten in place as the stored-block frame.
+//   sky_verify_index_kernel  : one thread per chunk.  FLG and BD must be exactly what write_frame_header (frame.cuh) writes
+//                              for the chunk and the batch's flags, then frame_index (lz4dec.cuh) checks magic, content
+//                              size and HC byte and walks the block words with nblk taken from the chunk's length; the
+//                              EndMark must follow the last block, the frame must end right behind it (and its content
+//                              checksum), and the content checksum must be the XXH32 the MD5 lanes computed from the chunk.
+//   sky_verify_kernel        : one warp per 64 KiB block, claimed row-major (claim_row_major, lz4dec.cuh).  The block
+//                              checksum over the block's stored bytes, then a stored block's bytes against the chunk, or a
+//                              compare-decode of a compressed block against the chunk.
+//   sky_verify_settle_kernel : one CTA per chunk.  The chunk's status (settle_status), and for a failing chunk with repair
+//                              on, its frame rewritten in place as the stored-block frame through frame.cuh's writers.
 // Compare-decode.  An independent block decodes to the source block iff every literal byte equals the source at its output
 // position q and every match byte satisfies src[q] == src[q - off]: by induction over q, once every output byte before q
 // equals the source, a match copies source bytes.  So no output buffer and no digest are needed, and every block checks
@@ -20,7 +19,8 @@
 // q - off >= the block start, no overrun of the block or of the block's bytes, a decoded length of exactly
 // min(64 KiB, n - block start), the last 5 bytes literals and the last match starting >= 12 bytes before the block end.
 // Status 0 therefore means liblz4 decodes the frame to the chunk.  A failure is reported in the receiver's codes, plus
-// kVerifyMismatch: well formed, but other bytes; within a chunk the earliest failing block's code wins (block_fail).
+// kVerifyMismatch: well formed, but other bytes; within a chunk the earliest failing block's code wins (block_fail, the
+// receiver's per-block status protocol in lz4dec.cuh).
 #pragma once
 #include <stdint.h>
 
@@ -50,24 +50,21 @@ struct VerifyParams {
     uint32_t repair;           // 1: rewrite failing frames
 };
 
-// The FLG bits the batch's checksum flags add to 0x68 (0x60 for an empty chunk): C.Checksum 0x04, B.Checksum 0x10
-__device__ __forceinline__ uint32_t stage_flg(uint32_t flags) {
-    return ((flags & SKY_F_CHECKSUM) ? 0x04u : 0u) | ((flags & SKY_F_BLOCK_CHECKSUM) ? 0x10u : 0u);
-}
-
 // One thread per chunk: the frame-level checks.  -> kDecOk, kDecChecksum (content checksum: the blocks are still checked,
 // and a block failure takes precedence) or a frame-level code (the blocks are not checked).
 __device__ __forceinline__ int32_t verify_frame(const VerifyParams &p, uint32_t c) {
     const ChunkDesc cd = p.chunks[c];
     DecChunk d{cd.dst, nullptr, p.frame_len[c], cd.len, p.blk_base[c], cd.nblk, 0, 0, 0};
     const uint8_t *f = cd.dst;
-    if (d.frame_len >= 11 && (f[4] != ((cd.len ? 0x68u : 0x60u) | stage_flg(p.flags)) || f[5] != 0x40)) return kDecBadHeader;
+    uint8_t want[kFrameHeaderBytes];  // the header the stage writes for this chunk
+    write_frame_header(want, cd.len, p.flags);
+    if (d.frame_len >= 11 && (f[4] != want[4] || f[5] != want[5])) return kDecBadHeader;
     int32_t st = kDecOk;
     frame_index(d, p.blocks + d.blk_base, &st);
     if (st != kDecOk) return st;
     // frame_index has found the EndMark behind block nblk - 1 (and room for the content checksum): the frame ends there
     const uint32_t bc = (p.flags & SKY_F_BLOCK_CHECKSUM) ? 4u : 0u;
-    uint64_t end = cd.len ? kFrameHeaderBytes : 7u;
+    uint64_t end = frame_header_bytes(cd.len);
     if (cd.nblk) {
         const DecBlock last = p.blocks[d.blk_base + cd.nblk - 1];
         end = last.off + (last.word & 0x7FFFFFFFu) + bc;
@@ -96,17 +93,6 @@ __device__ __forceinline__ bool warp_equal(const uint8_t *a, const uint8_t *s, u
     }
     for (uint32_t k = (nvec << 4) + lane; k < n; k += 32) ok &= a[k] == s[k];
     return __all_sync(kFull, ok);
-}
-
-// Length extension of a 4-bit field that reads 15; false when it runs off the block's bytes.
-__device__ __forceinline__ bool read_ext(const uint8_t *blk, uint32_t slen, uint32_t &ip, uint32_t &len) {
-    uint32_t s;
-    do {
-        if (ip >= slen) return false;
-        s = blk[ip++];
-        len += s;
-    } while (s == 255 && len < (1u << 24));
-    return true;
 }
 
 // Whole warp, warp-uniform arguments: compare-decode of the compressed block blk[0, slen) against its source block
@@ -165,57 +151,47 @@ __global__ void sky_verify_index_kernel(const VerifyParams p) {
 // of its chunk has failed.
 __global__ void __launch_bounds__(kVerifyThreads, 2) sky_verify_kernel(const VerifyParams p) {
     const unsigned lane = threadIdx.x & 31;
-    const uint32_t total = p.rows * p.n_chunks;
     const bool bc = (p.flags & SKY_F_BLOCK_CHECKSUM) != 0;
-    for (;;) {
-        uint32_t w = 0;
-        if (lane == 0) w = atomicAdd(p.counter, 1u);
-        w = __shfl_sync(kFull, w, 0);
-        if (w >= total) break;
-        const uint32_t c = w % p.n_chunks, j = w / p.n_chunks;
+    for (uint32_t c, j; claim_row_major(p.counter, p.n_chunks, p.rows, lane, c, j);) {
         const ChunkDesc cd = p.chunks[c];
         if (j >= cd.nblk) continue;
-        const int32_t st = *reinterpret_cast<volatile int32_t *>(p.status + c);
-        if (!(st == kDecOk || st == kDecChecksum || (st < kDecChecksum && st > block_fail(j, 0)))) continue;
+        if (!block_may_run(*reinterpret_cast<volatile int32_t *>(p.status + c), j)) continue;
         const int32_t r = verify_block(cd, p.blocks[p.blk_base[c] + j], j, bc, lane);
         if (r != kDecOk && lane == 0) atomicMin(p.status + c, block_fail(j, r));
     }
 }
 
 // One CTA per chunk: settle the status; with repair, rewrite a failing frame in place as the chunk's stored-block frame --
-// the stage's header, every block stored raw from the chunk (with its block checksum under SKY_F_BLOCK_CHECKSUM), the
-// EndMark and the content checksum (finish_frame) -- frame_need(n, flags) bytes, which the frame's capacity holds.
+// the stage's header (write_frame_header), every block stored raw from the chunk (with its block checksum under
+// SKY_F_BLOCK_CHECKSUM), the EndMark and the content checksum (finish_frame) -- frame_need(n, flags) bytes, which the
+// frame's capacity holds.
 __global__ void __launch_bounds__(kRepairWarps * 32) sky_verify_settle_kernel(const VerifyParams p) {
     __shared__ int32_t code;
     const uint32_t c = blockIdx.x;
     const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        const int32_t s = p.status[c];
-        code = s < kDecChecksum ? -((s - kBlockFail) & 15) : s;
+        code = settle_status(p.status[c]);
         p.status_out[c] = code;
     }
     __syncthreads();
     if (code == kDecOk || !p.repair) return;
     const ChunkDesc cd = p.chunks[c];
     const uint32_t bc = (p.flags & SKY_F_BLOCK_CHECKSUM) ? 4u : 0u;
-    const uint64_t hdr = cd.len ? kFrameHeaderBytes : 7u;
+    const uint64_t hdr = frame_header_bytes(cd.len);
     for (uint32_t j = 0; j < cd.nblk; j++) {
         const uint64_t pos = (uint64_t)j * kBlock;
         const uint32_t L = (uint32_t)min((uint64_t)kBlock, cd.len - pos);
         uint8_t *w = cd.dst + hdr + (uint64_t)j * (4 + kBlock + bc);
-        if (threadIdx.x == 0) {
-            const uint32_t hword = L | 0x80000000u;
-            w[0] = (uint8_t)hword; w[1] = (uint8_t)(hword >> 8); w[2] = (uint8_t)(hword >> 16); w[3] = (uint8_t)(hword >> 24);
-        }
+        if (threadIdx.x == 0) st_u32le(w, L | 0x80000000u);
         copy_block<kRepairWarps, true>(w + 4, cd.src + pos, L, warp, lane);
         if (bc && warp == j % kRepairWarps) block_checksum(cd.src + pos, L, w + 4 + L, lane);  // (the same bytes, from the chunk)
     }
     if (threadIdx.x == 0) {
-        write_frame_header(cd.dst, cd.len);
+        write_frame_header(cd.dst, cd.len, p.flags);
         uint8_t *e = cd.dst + hdr + (uint64_t)cd.nblk * (4 + bc) + cd.len;
-        e[0] = e[1] = e[2] = e[3] = 0;  // EndMark
+        st_u32le(e, 0);  // EndMark
         p.frame_len[c] = (uint64_t)(e - cd.dst) + 4;
-        finish_frame(p.chunks, (p.flags & SKY_F_CHECKSUM) ? p.xxh : nullptr, p.frame_len, c, stage_flg(p.flags));
+        if (p.flags & SKY_F_CHECKSUM) finish_frame(cd.dst, p.frame_len + c, p.xxh[c]);
     }
 }
 

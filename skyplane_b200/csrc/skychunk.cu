@@ -402,11 +402,11 @@ __global__ void __launch_bounds__(kThreads, 2) sky_fused_xxh_kernel(const Params
 __global__ void __launch_bounds__(kThreads, 2) sky_fused_bc_kernel(const Params p) { fused_body<false, true>(p); }
 __global__ void __launch_bounds__(kThreads, 2) sky_fused_xxh_bc_kernel(const Params p) { fused_body<true, true>(p); }
 
-// Frame-descriptor epilogue (finish_frame, frame.cuh), one thread per chunk, after the compressor has finished the frame.
-__global__ void sky_checksum_kernel(const ChunkDesc *chunks, const uint32_t *xxh, uint64_t *out_len, uint32_t n, uint32_t flg) {
+// SKY_F_CHECKSUM epilogue (finish_frame, frame.cuh), one thread per chunk, after the compressor has finished the frame.
+__global__ void sky_checksum_kernel(const ChunkDesc *chunks, const uint32_t *xxh, uint64_t *out_len, uint32_t n) {
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= n) return;
-    finish_frame(chunks, xxh, out_len, c, flg);
+    finish_frame(chunks[c].dst, out_len + c, xxh[c]);
 }
 
 
@@ -476,11 +476,11 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
             }
             const uint32_t x = md5_warp<true>(reinterpret_cast<uint32_t *>(smem + warp * kRingBytes), src, len, active,
                                               p.md5_out + (size_t)(active ? c : 0) * 16, lane, gate);
-            // every row has passed the gate, so no decode warp writes the status any more: settle a block failure into its
-            // code (lz4dec.cuh, block_fail); a content checksum mismatch only replaces ok
+            // every row has passed the gate, so no decode warp reads or writes the status any more: settle a block failure
+            // into its code (lz4dec.cuh); a content checksum mismatch only replaces ok
             if (active) {
-                const int32_t s = *reinterpret_cast<volatile int32_t *>(p.status + c);
-                if (s < kDecChecksum) p.status[c] = -((s - kBlockFail) & 15);
+                const int32_t s = settle_status(*reinterpret_cast<volatile int32_t *>(p.status + c));
+                if (s != kDecOk) p.status[c] = s;
                 else if ((p.chunks[c].checks & kChkContent) && x != p.chunks[c].content_xxh) atomicCAS(p.status + c, kDecOk, kDecChecksum);
             }
             __syncwarp();
@@ -489,13 +489,7 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
     // A failing block folds block_fail(j, code) into the chunk's status with atomicMin, so the earliest failing block wins
     // whichever warp gets there first (liblz4 checks and decodes blocks in order and reports the first error); the chunk's
     // MD5 lane turns it back into that block's code.  A block is skipped only once the header or an earlier block failed.
-    const uint32_t total = p.rows * p.n_chunks;
-    for (;;) {
-        uint32_t w = 0;
-        if (lane == 0) w = atomicAdd(p.counter, 1u);
-        w = __shfl_sync(kFull, w, 0);
-        if (w >= total) break;
-        const uint32_t c = w % p.n_chunks, j = w / p.n_chunks;
+    for (uint32_t c, j; claim_row_major(p.counter, p.n_chunks, p.rows, lane, c, j);) {
         const DecChunk cd = p.chunks[c];
         if (j >= cd.nblk) continue;
         int32_t st = *reinterpret_cast<volatile int32_t *>(p.status + c);
@@ -512,7 +506,7 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
             __syncwarp();
             st = *reinterpret_cast<volatile int32_t *>(p.status + c);
         }
-        if (st == kDecOk || (st < kDecChecksum && st > block_fail(j, 0))) {  // no failure yet, or only in later blocks
+        if (block_may_run(st, j)) {
             const DecBlock b = p.blocks[cd.blk_base + j];
             const uint32_t sz = b.word & 0x7FFFFFFFu;
             if ((cd.checks & kChkBlock) && xxh32_warp(cd.frame + b.off, sz, lane) != b.chk) {
@@ -633,13 +627,14 @@ static int hc_level(uint32_t flags) {
     const int l = (int)((flags & kHcLevelMask) >> kHcLevelShift);
     return l ? l : kHcDefaultLevel;
 }
+struct BlockTable {  // per block of a batch, `cap` entries: what frame_index found; done = decoded (the receiver's MD5 gate)
+    DevMem<DecBlock> blocks; DevMem<uint32_t> done; uint64_t cap = 0;
+};
 struct DecodeArrays {  // receiver side
     PinnedMem<DecChunk> h_chunks; DevMem<DecChunk> d_chunks;
     PinnedMem<int32_t> h_status; DevMem<int32_t> d_status;
     DevMem<uint32_t> d_dec_done;  // per chunk: leading blocks decoded (linked frames wait on it)
-    DevMem<DecBlock> d_blocks;    // per block of the batch: blocks_cap entries, grown on demand
-    DevMem<uint32_t> d_blk_done;
-    uint64_t blocks_cap = 0;
+    BlockTable table;
 };
 struct BoxArrays {  // E2EE: box slab, per-chunk box descriptors, stream-block prefix, subkeys, nonces, tag verdicts
     DevMem<uint8_t> d_box;
@@ -654,8 +649,7 @@ struct VerifyArrays {  // SKY_F_VERIFY: block-table bases, statuses (device, and
     DevMem<int32_t> d_status;
     Mapped<int32_t> status;
     DevMem<uint32_t> d_counter;
-    DevMem<DecBlock> d_blocks;  // per block of the batch: blocks_cap entries, grown on demand
-    uint64_t blocks_cap = 0;
+    BlockTable table;
 };
 struct Ticket {  // the batch a slot has in flight on the host path
     bool busy = false, d2h_issued = false;
@@ -780,6 +774,16 @@ static int alloc_verify(sky_ctx *ctx, VerifyArrays &v) {
     CK(ctx, a.status.alloc(nc));
     CK(ctx, cudaMalloc(a.d_counter.put(), sizeof(uint32_t)));
     v = std::move(a);
+    return SKY_OK;
+}
+
+static int grow_block_table(sky_ctx *ctx, cudaStream_t st, BlockTable &t, uint64_t n) {
+    if (n <= t.cap) return SKY_OK;
+    CK(ctx, cudaStreamSynchronize(st));  // kernels queued earlier on `st` are done with the old arrays
+    t.cap = 0;
+    CK(ctx, cudaMalloc(t.blocks.put(), n * sizeof(DecBlock)));
+    CK(ctx, cudaMalloc(t.done.put(), n * sizeof(uint32_t)));
+    t.cap = n;
     return SKY_OK;
 }
 
@@ -1049,12 +1053,8 @@ static int launch_verify(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, uin
         v.h_blk_base[i] = nblk_total;
         nblk_total += m.h_desc[i].nblk;
     }
-    if (nblk_total + 1 > v.blocks_cap) {
-        CK(ctx, cudaStreamSynchronize(st));  // an earlier check is done with the old table
-        v.blocks_cap = 0;
-        CK(ctx, cudaMalloc(v.d_blocks.put(), (nblk_total + 1) * sizeof(DecBlock)));
-        v.blocks_cap = nblk_total + 1;
-    }
+    rc = grow_block_table(ctx, st, v.table, nblk_total + 1);
+    if (rc != SKY_OK) return rc;
     CK(ctx, cudaMemcpyAsync(v.d_blk_base, v.h_blk_base, n * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
     CK(ctx, cudaMemsetAsync(v.d_counter, 0, sizeof(uint32_t), st));
     VerifyParams p;
@@ -1062,7 +1062,7 @@ static int launch_verify(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, uin
     p.frame_len = m.outlen.d;
     p.xxh = (flags & SKY_F_CHECKSUM) ? (const uint32_t *)m.xxh : nullptr;
     p.blk_base = v.d_blk_base;
-    p.blocks = v.d_blocks;
+    p.blocks = v.table.blocks;
     p.status = v.d_status;
     p.status_out = v.status.d;
     p.counter = v.d_counter;
@@ -1158,9 +1158,8 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
         CK(ctx, cudaGetLastError());
     }
     ctx->launches++;
-    if (xxh || bc) {  // FLG and the header checksum byte of every frame, and the content checksum
-        sky_checksum_kernel<<<(n + 127) / 128, 128, 0, st>>>(m.d_desc, xxh ? (const uint32_t *)m.xxh : nullptr, m.outlen.d, n,
-                                                             (xxh ? 0x04u : 0u) | (bc ? 0x10u : 0u));
+    if (xxh) {  // the content checksum behind every frame's EndMark
+        sky_checksum_kernel<<<(n + 127) / 128, 128, 0, st>>>(m.d_desc, m.xxh, m.outlen.d, n);
         CK(ctx, cudaGetLastError());
         ctx->launches++;
     }
@@ -1381,30 +1380,24 @@ static int launch_decode(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, con
         d.h_chunks[i] = DecChunk{d_frames + frame_off[i], d_out + out_off[i], frame_len[i], raw_len[i], nblk_total, nblk, 0};
         nblk_total += nblk;
     });
+    if (rc == SKY_OK) rc = grow_block_table(ctx, st, d.table, nblk_total + 1);
     if (rc != SKY_OK) return rc;
-    if (nblk_total + 1 > d.blocks_cap) {
-        CK(ctx, cudaStreamSynchronize(st));  // the previous decode is done with the old arrays
-        d.blocks_cap = 0;
-        CK(ctx, cudaMalloc(d.d_blocks.put(), (nblk_total + 1) * sizeof(DecBlock)));
-        CK(ctx, cudaMalloc(d.d_blk_done.put(), (nblk_total + 1) * sizeof(uint32_t)));
-        d.blocks_cap = nblk_total + 1;
-    }
     BatchMeta &m = s.meta;
     CK(ctx, cudaMemcpyAsync(d.d_chunks, d.h_chunks, n * sizeof(DecChunk), cudaMemcpyHostToDevice, st));
     CK(ctx, cudaMemsetAsync(m.counters, 0, 64, st));
     CK(ctx, cudaMemsetAsync(d.d_dec_done, 0, n * sizeof(uint32_t), st));
     CK(ctx, cudaMemsetAsync(d.d_status, 0, n * sizeof(int32_t), st));
-    CK(ctx, cudaMemsetAsync(d.d_blk_done, 0, (nblk_total + 1) * sizeof(uint32_t), st));
+    CK(ctx, cudaMemsetAsync(d.table.done, 0, (nblk_total + 1) * sizeof(uint32_t), st));
     const uint32_t ng = fill_md5_order(m.h_order, n, raw_len);
     CK(ctx, cudaMemcpyAsync(m.d_order, m.h_order, ng * 32 * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     memset(m.md5.h, 0, (size_t)n * 16);
     DecParams p;
     p.chunks = d.d_chunks;
-    p.blocks = d.d_blocks;
+    p.blocks = d.table.blocks;
     p.status = d.d_status;
     p.dec_done = d.d_dec_done;
     p.counter = m.counters;
-    p.blk_done = d.d_blk_done;
+    p.blk_done = d.table.done;
     p.md5_order = m.d_order;
     p.md5_out = m.md5.d;
     p.n_chunks = n;

@@ -19,8 +19,9 @@ pytestmark = pytest.mark.skipif(not ref.available(), reason="liblz4.so.1 not fou
 
 
 def with_content_checksum(frame: bytes, data: bytes) -> bytes:
-    """What sky_checksum_kernel does to a finished frame (FLG 0x68 / 0x60): set C.Checksum, recompute the header checksum
-    byte over the descriptor, append u32le XXH32(chunk) behind the EndMark."""
+    """The stage's SKY_F_CHECKSUM frame from the same frame without the flag (FLG 0x68 / 0x60): C.Checksum set and the
+    header checksum byte over that descriptor (the compressor writes this header), u32le XXH32(chunk) behind the EndMark
+    (sky_checksum_kernel appends it)."""
     dlen = 10 if data else 2
     f = bytearray(frame)
     f[4] |= 0x04

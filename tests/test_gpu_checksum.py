@@ -153,7 +153,10 @@ def test_flag_rules(ctx):
     run_device(ctx, datas, 0)
     n1 = ctx.launches
     run_device(ctx, datas, CK)
-    assert n1 - n0 == 1 and ctx.launches - n1 == 2  # the checksum epilogue only when asked for
+    n2 = ctx.launches
+    run_device(ctx, datas, native.F_BLOCK_CHECKSUM, 4 * 5)  # (5 blocks in the longest chunk)
+    assert n1 - n0 == 1 and n2 - n1 == 2  # the checksum epilogue only when asked for
+    assert ctx.launches - n2 == 1  # block checksums need no epilogue: the compressor writes the final header
 
 
 def test_e2ee_seals_the_checksummed_frame(stage):
