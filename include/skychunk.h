@@ -173,9 +173,27 @@ SKY_API int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, cons
  * error status, never a crash); md5[16*i..] = MD5 of the decoded bytes.
  * sky_decode_device: frames and output already in HBM (out_off multiples of 16; each frame region must be readable
  * up to the next multiple of 4 bytes, each output region writable up to the next multiple of 16).  sky_decode: host
- * buffers, synchronous, through slot 0's slabs (needs n_slots >= 1); flags = 0, or SKY_F_E2EE: the payloads are sealed
- * boxes, whose tags are checked and which are opened on the device before the frames are decoded (status SKY_D_AUTH for
- * a forged / truncated box, whose bytes are never returned). */
+ * buffers, synchronous, through slot 0's slabs (needs n_slots >= 1).  Its flags are the stage bits the sender's
+ * sky_submit was given, so every payload sky_submit makes has a receiver:
+ *
+ *     sky_submit flags                what is on the wire             sky_decode flags
+ *     0 / SKY_F_LZ4 | SKY_F_MD5       LZ4 frame                       0 (or SKY_F_LZ4, SKY_F_LZ4 | SKY_F_MD5)
+ *     ... | SKY_F_E2EE                SecretBox of the frame          SKY_F_E2EE (with or without the two bits)
+ *     SKY_F_MD5 (`compress: false`)   the chunk's own bytes           SKY_F_MD5
+ *     SKY_F_MD5 | SKY_F_E2EE          SecretBox of the chunk          SKY_F_MD5 | SKY_F_E2EE
+ *
+ * SKY_F_E2EE: the payloads are sealed boxes, whose tags are checked and which are opened on the device first (status
+ * SKY_D_AUTH for a forged / truncated box, whose bytes are never returned; SKY_E_NOKEY without a key).
+ * SKY_F_MD5 alone: payload i IS chunk i (WireProtocolHeader.is_compressed = False): frames[i] / frame_len[i] are the
+ * received bytes, raw_len[i] the header's raw_data_len; frame_len[i] != raw_len[i] is SKY_D_SIZE (the size check of
+ * gateway_receiver.py:213-218).  The chunks are digested on the device by the launch sky_submit(SKY_F_MD5) makes and
+ * nothing is copied back: dst may be NULL and a dst[i] is not written, as sky_submit(SKY_F_MD5) writes no dst.
+ * SKY_F_MD5 | SKY_F_E2EE: every box is opened straight into the digest's input; the opened chunk is copied to dst[i]
+ * (needed when raw_len[i] > 0).  An authentic box whose message is not raw_len[i] bytes long is SKY_D_SIZE and is not
+ * copied out; SKY_D_AUTH comes before SKY_D_SIZE.  In both raw modes the digest of a chunk whose status is not 0 is 16 zero
+ * bytes, and kernel_ms covers open + digest.  Any other flag bit is SKY_E_INVALID: a frame says itself which checksums
+ * it carries and any compressor's frames decode alike, so the receiver has no frame option to take.
+ * sky_decode_device takes no flags: for chunks already in HBM, receiving a raw chunk is sky_process_device(SKY_F_MD5). */
 #define SKY_D_OK 0
 #define SKY_D_BAD_HEADER (-1)
 #define SKY_D_CORRUPT (-2)

@@ -643,6 +643,7 @@ struct BoxArrays {  // E2EE: box slab, per-chunk box descriptors, stream-block p
     DevMem<uint32_t> d_sub;
     PinnedMem<uint8_t> h_nonce; DevMem<uint8_t> d_nonce;
     PinnedMem<int32_t> h_status; DevMem<int32_t> d_status;
+    Event ev_open;  // the boxes are on the device, the open kernels start (kernel_ms of a batch of sealed raw chunks)
 };
 struct VerifyArrays {  // SKY_F_VERIFY: block-table bases, statuses (device, and settled in mapped host memory), block table
     PinnedMem<uint64_t> h_blk_base; DevMem<uint64_t> d_blk_base;
@@ -801,6 +802,7 @@ static int alloc_box(sky_ctx *ctx, BoxArrays &b) {
     CK(ctx, cudaMalloc(a.d_nonce.put(), nc * 24));
     CK(ctx, cudaMallocHost(a.h_status.put(), nc * sizeof(int32_t)));
     CK(ctx, cudaMalloc(a.d_status.put(), nc * sizeof(int32_t)));
+    CK(ctx, cudaEventCreate(a.ev_open.put()));
     b = std::move(a);
     return SKY_OK;
 }
@@ -986,25 +988,28 @@ static int launch_seal(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, uint8
     return SKY_OK;
 }
 
-// Open the n boxes on slot `s`: copy box i to the box slab at frame_off[i] + 64 * i + 8, and open it into the frame slab at
-// frame_off[i] (msg_len[i] = its message bytes): keys -> tag -> xor, then the tag verdicts to the host.  Every offset and
-// length is known before the kernels run, so the host writes the descriptors.
-static int launch_open(sky_ctx *ctx, Slot &s, uint32_t n, const void *const *boxes, const uint64_t *box_len, const uint64_t *frame_off,
-                       uint64_t *msg_len) {
+// Open the n boxes on slot `s`: copy box i to the box slab at box_off[i] + 64 * i + 8 (box_off: 16-byte aligned, at least
+// box_len[i] apart), and open it into d_msg + msg_off[i] (16-byte aligned; msg_len[i] = its message bytes) -- the frame
+// slab when the messages are frames to decode, the input slab when they are the chunks themselves: keys -> tag -> xor,
+// then the tag verdicts to the host.  Every offset and length is known before the kernels run, so the host writes the
+// descriptors.
+static int launch_open(sky_ctx *ctx, Slot &s, uint32_t n, const void *const *boxes, const uint64_t *box_len, const uint64_t *box_off,
+                       uint8_t *d_msg, const uint64_t *msg_off, uint64_t *msg_len) {
     BoxArrays &b = s.box;
     const cudaStream_t st = s.stream;
     uint64_t acc = 0;
     for (uint32_t i = 0; i < n; i++) {
-        uint8_t *box = b.d_box + frame_off[i] + 64ull * i + 8;
+        uint8_t *box = b.d_box + box_off[i] + 64ull * i + 8;
         CK(ctx, cudaMemcpyAsync(box, boxes[i], box_len[i], cudaMemcpyHostToDevice, st));
         msg_len[i] = box_len[i] >= (uint64_t)kBoxOverhead ? box_len[i] - kBoxOverhead : 0;
-        b.h_chunks[i] = BoxChunk{box, s.d_out + frame_off[i], msg_len[i]};
+        b.h_chunks[i] = BoxChunk{box, d_msg + msg_off[i], msg_len[i]};
         b.h_blk_base[i] = acc;
         acc += box_stream_blocks(msg_len[i]);
     }
     b.h_blk_base[n] = acc;
     CK(ctx, cudaMemcpyAsync(b.d_chunks, b.h_chunks, n * sizeof(BoxChunk), cudaMemcpyHostToDevice, st));
     CK(ctx, cudaMemcpyAsync(b.d_blk_base, b.h_blk_base, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    CK(ctx, cudaEventRecord(b.ev_open, st));
     sky_box_keys_kernel<<<(n + 63) / 64, 64, 0, st>>>(b.d_chunks, n, ctx->d_key, b.d_sub);
     CK(ctx, cudaGetLastError());
     sky_box_tag_kernel<<<n, kPolyThreads, 0, st>>>(b.d_chunks, b.d_sub, 1, b.d_status);
@@ -1437,16 +1442,65 @@ int sky_decode_device(sky_ctx *ctx, uint32_t n, const void *d_frames, const uint
     return SKY_OK;
 }
 
+// sky_decode of payloads that are the chunks themselves (SKY_F_MD5 alone: the sender's `compress: false`), sealed or not.
+// The chunk bytes go into the slot's INPUT slab -- copied there, or opened there from their boxes -- and are digested by
+// the launch sky_submit(SKY_F_MD5) makes.  A chunk of the wrong size is left out of that launch (length 0), and the digest of a
+// chunk that fails is reported as 16 zero bytes.  Only opened chunks are copied back: an unsealed one the caller already holds.
+static int decode_raw(sky_ctx *ctx, Slot &s, uint32_t n, const void *const *payload, const uint64_t *payload_len, void *const *dst,
+                      const uint64_t *raw_len, bool e2ee, int32_t *status, uint8_t *md5, float *kernel_ms) {
+    std::vector<uint64_t> off(n), box_off(n), msg_len(payload_len, payload_len + n), md5_len(n);
+    uint64_t ip = 0, bp = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        if (payload_len[i] && !payload[i]) return SKY_E_INVALID;
+        if (e2ee && raw_len[i] && !dst[i]) return SKY_E_INVALID;
+        if (e2ee) msg_len[i] = payload_len[i] >= (uint64_t)kBoxOverhead ? payload_len[i] - kBoxOverhead : 0;
+        md5_len[i] = msg_len[i] == raw_len[i] ? raw_len[i] : 0;
+        off[i] = ip;
+        box_off[i] = bp;
+        ip += round16(e2ee ? msg_len[i] : md5_len[i]);  // (an opened chunk lands whole, whatever size was expected)
+        bp += round16(payload_len[i]);
+    }
+    if (ip > ctx->in_cap || (e2ee && bp > ctx->out_cap)) return SKY_E_CAPACITY;
+    if (e2ee) {
+        const int rc = launch_open(ctx, s, n, payload, payload_len, box_off.data(), s.d_in, off.data(), msg_len.data());
+        if (rc != SKY_OK) return rc;
+    } else {
+        for (uint32_t i = 0; i < n; i++)
+            if (md5_len[i]) CK(ctx, cudaMemcpyAsync(s.d_in + off[i], payload[i], md5_len[i], cudaMemcpyHostToDevice, s.stream));
+    }
+    // (no frames are written without SKY_F_LZ4: the frame slab only lends the descriptors an address)
+    int rc = launch_batch(ctx, s, s.stream, s.stream, n, s.d_in, off.data(), md5_len.data(), s.d_out, off.data(), SKY_F_MD5);
+    if (rc != SKY_OK) return rc;
+    CK(ctx, cudaStreamSynchronize(s.stream));
+    for (uint32_t i = 0; i < n; i++) {
+        int32_t st = msg_len[i] == raw_len[i] ? SKY_D_OK : SKY_D_SIZE;
+        if (e2ee && (s.box.h_status[i] != 0 || payload_len[i] < (uint64_t)kBoxOverhead)) st = SKY_D_AUTH;  // never hand its bytes out
+        if (status) status[i] = st;
+        if (md5) {
+            if (st == SKY_D_OK) memcpy(md5 + 16ull * i, s.meta.md5.h + 16ull * i, 16);
+            else memset(md5 + 16ull * i, 0, 16);
+        }
+        if (e2ee && st == SKY_D_OK && raw_len[i])
+            CK(ctx, cudaMemcpyAsync(dst[i], s.d_in + off[i], raw_len[i], cudaMemcpyDeviceToHost, s.stream));
+    }
+    if (e2ee) CK(ctx, cudaStreamSynchronize(s.stream));
+    if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, e2ee ? (cudaEvent_t)s.box.ev_open : (cudaEvent_t)s.ev_k0, s.ev_k1));  // open + digest
+    return SKY_OK;
+}
+
 int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64_t *frame_len, void *const *dst,
                const uint64_t *raw_len, uint32_t flags, int32_t *status, uint8_t *md5, float *kernel_ms) {
-    if (!ctx || n == 0 || !frames || !frame_len || !dst || !raw_len) return SKY_E_INVALID;
+    if (flags & ~(SKY_F_LZ4 | SKY_F_MD5 | SKY_F_E2EE)) return SKY_E_INVALID;  // a receiver takes what it is sent: no frame options
+    const bool e2ee = (flags & SKY_F_E2EE) != 0, raw = (flags & (SKY_F_LZ4 | SKY_F_MD5)) == SKY_F_MD5;
+    const bool returns_data = !raw || e2ee;  // an unsealed raw chunk is only digested: the caller holds its bytes
+    if (!ctx || n == 0 || !frames || !frame_len || (returns_data && !dst) || !raw_len) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
     Slot &s = ctx->slots[0];
     if (s.ticket.busy) return SKY_E_BUSY;
     if (!s.d_in) return SKY_E_INVALID;  // ctx created without slabs
-    const bool e2ee = (flags & SKY_F_E2EE) != 0;
     if (e2ee && !ctx->d_key) return SKY_E_NOKEY;
     CK(ctx, cudaSetDevice(ctx->device));
+    if (raw) return decode_raw(ctx, s, n, frames, frame_len, dst, raw_len, e2ee, status, md5, kernel_ms);
     // roles swap on the way back: frames (<= bound) go into the frame slab, decoded bytes into the input slab
     std::vector<uint64_t> f_off(n), o_off(n), f_len(frame_len, frame_len + n);
     uint64_t fp = 0, op = 0;
@@ -1460,7 +1514,7 @@ int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64
     if (fp > ctx->out_cap || op > ctx->in_cap) return SKY_E_CAPACITY;
     if (e2ee) {
         // the payloads are boxes (nonce | tag | ciphertext): check the tags, decrypt into the frame slab, then decode as usual
-        int rc = launch_open(ctx, s, n, frames, frame_len, f_off.data(), f_len.data());
+        int rc = launch_open(ctx, s, n, frames, frame_len, f_off.data(), s.d_out, f_off.data(), f_len.data());
         if (rc != SKY_OK) return rc;
     } else {
         for (uint32_t i = 0; i < n; i++)

@@ -195,6 +195,21 @@ def frame_need(n: int, checksum: bool = False, block_checksum: bool = False) -> 
     return frame_bound(n) + (CHECKSUM_BYTES if checksum else 0) + (CHECKSUM_BYTES * blocks if block_checksum else 0)
 
 
+_DECODE_ONLY_SUBMIT = ((F_HC, "F_HC"), (HC_LEVEL_MASK, "a high-ratio level"), (F_CHECKSUM, "F_CHECKSUM"),
+                       (F_BLOCK_CHECKSUM, "F_BLOCK_CHECKSUM"), (F_VERIFY, "F_VERIFY"))
+
+
+def check_decode_flags(flags: int) -> int:
+    """sky_decode takes the stage bits (F_LZ4, F_MD5) and F_E2EE only: a frame says itself which checksums it carries, and
+    the compressor that made it does not matter to a decoder.  -> flags, or a ValueError naming the bit it does not take."""
+    for bit, name in _DECODE_ONLY_SUBMIT:
+        if flags & bit:
+            raise ValueError(f"decode does not take {name}: it is a sender option (flags {flags:#x})")
+    if flags & ~(F_LZ4 | F_MD5 | F_E2EE):
+        raise ValueError(f"decode does not know flag bits {flags & ~(F_LZ4 | F_MD5 | F_E2EE):#x}")
+    return flags
+
+
 def round16(x: int) -> int:
     return (x + 15) & ~15
 
@@ -364,15 +379,20 @@ class Context:
         raw = bytes(md5)
         return list(st), [raw[16 * i : 16 * i + 16] for i in range(n)], ms.value
 
-    def decode(self, frame_addrs: Sequence[int], frame_lens: Sequence[int], dst_addrs: Sequence[int], raw_lens: Sequence[int], flags: int = 0):
-        """Host buffers, synchronous. -> (status, digests, kernel_ms).  flags = F_E2EE: the payloads are sealed boxes."""
+    def decode(self, frame_addrs: Sequence[int], frame_lens: Sequence[int], dst_addrs: Optional[Sequence[int]], raw_lens: Sequence[int],
+               flags: int = 0):
+        """Host buffers, synchronous. -> (status, digests, kernel_ms).  flags: the sender's stage bits (check_decode_flags).
+        0: LZ4 frames; F_MD5: the payloads are the chunks themselves (`compress: false`), which are only digested -- nothing
+        is written, dst_addrs may be None; | F_E2EE: the payloads are sealed boxes, and what they hold comes back in dst."""
+        check_decode_flags(flags)
         n = len(frame_addrs)
         A = ctypes.c_void_p * n
         U = ctypes.c_uint64 * n
         st = (ctypes.c_int32 * n)()
         md5 = (ctypes.c_ubyte * (16 * n))()
         ms = ctypes.c_float(0)
-        self._check(lib().sky_decode(self._h, n, A(*frame_addrs), U(*frame_lens), A(*dst_addrs), U(*raw_lens), flags, st, md5, ctypes.byref(ms)))
+        self._check(lib().sky_decode(self._h, n, A(*frame_addrs), U(*frame_lens), A(*dst_addrs) if dst_addrs is not None else None,
+                                     U(*raw_lens), flags, st, md5, ctypes.byref(ms)))
         raw = bytes(md5)
         return list(st), [raw[16 * i : 16 * i + 16] for i in range(n)], ms.value
 

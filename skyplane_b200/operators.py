@@ -476,11 +476,20 @@ class GatewayDecompressVerify(GatewayOperator):
     with ``chunk.md5_hash`` when the sender supplied one.  Requests are drained in batches (one decode launch per batch);
     a payload that is missing or still being written is re-queued like GatewayWaitReceiver does (gateway_operator.py:131-150);
     a complete but corrupt payload, a forged box or a digest mismatch raises, which stops the gateway through
-    ``error_event`` like any other operator failure."""
+    ``error_event`` like any other operator failure.
+
+    ``use_compression=False`` is the receiving side of ``GatewayCompressHash(use_compression=False)`` (the reference's
+    ``compress: false``, ``is_compressed = False`` on the wire): there is no frame to decode.  With a key the payload
+    ``<chunk_id>.chunk.lz4`` is the SecretBox of the chunk: it is opened and digested on the GPU and written as
+    ``<chunk_id>.chunk``.  Without a key the payload is the chunk, which the receiver has already written as
+    ``<chunk_id>.chunk`` (gateway_receiver.py:204-224): that file is read, digested on the GPU and compared with
+    ``chunk.md5_hash``, and is not rewritten; while its size is not ``chunk_length_bytes`` it counts as still arriving."""
 
     def __init__(self, *args, max_batch_chunks: int = 64, max_batch_bytes: int = 512 << 20, n_gpus: Optional[int] = None,
-                 remove_frames: bool = True, e2ee_key_bytes: Optional[bytes] = None, stale_retries: int = 50, **kwargs):
+                 remove_frames: bool = True, e2ee_key_bytes: Optional[bytes] = None, stale_retries: int = 50,
+                 use_compression: bool = True, **kwargs):
         super().__init__(*args, **kwargs)
+        self.use_compression = True if use_compression is None else bool(use_compression)
         self.max_batch_chunks = max_batch_chunks
         self.max_batch_bytes = max_batch_bytes
         self.n_gpus = n_gpus
@@ -526,8 +535,11 @@ class GatewayDecompressVerify(GatewayOperator):
         ok = [False] * len(reqs)
         ready, frames = [], []
         total = 0
+        encrypted = self.e2ee_key_bytes is not None
+        in_place = not self.use_compression and not encrypted  # the payload is the chunk: <chunk_id>.chunk, digested where it lies
+        payload_path = self.chunk_store.get_chunk_file_path if in_place else self.chunk_store.get_compressed_file_path
         for i, r in enumerate(reqs):
-            fpath = self.chunk_store.get_compressed_file_path(r.chunk.chunk_id)
+            fpath = payload_path(r.chunk.chunk_id)
             try:
                 frame = fpath.read_bytes()
             except FileNotFoundError:
@@ -539,12 +551,14 @@ class GatewayDecompressVerify(GatewayOperator):
             frames.append(frame)
         if not ready:
             return ok
-        encrypted = self.e2ee_key_bytes is not None
-        out = self._get_stage().decode(frames, [reqs[i].chunk.chunk_length_bytes for i in ready], encrypted=encrypted)
+        raw = {} if self.use_compression else {"compressed": False}
+        out = self._get_stage().decode(frames, [reqs[i].chunk.chunk_length_bytes for i in ready], encrypted=encrypted, **raw)
+        arriving = (native.D_TRUNCATED, native.D_BAD_HEADER, native.D_AUTH) + ((native.D_SIZE,) if in_place else ())
         for i, frame, (data, digest, status) in zip(ready, frames, out):
             chunk = reqs[i].chunk
-            if status in (native.D_TRUNCATED, native.D_BAD_HEADER, native.D_AUTH) and self._still_arriving(chunk.chunk_id, len(frame)):
-                continue  # a writer may still be appending (a short box fails authentication, a short frame is truncated)
+            if status in arriving and self._still_arriving(chunk.chunk_id, len(frame)):
+                continue  # a writer may still be appending (a short box fails authentication, a short frame is truncated,
+                #           a short chunk file has the wrong size)
             if status == native.D_CHECKSUM:  # complete frame whose block or content checksum fails: never "still arriving"
                 raise ChecksumMismatchException(f"chunk {chunk.chunk_id}: LZ4 frame checksum does not match the decoded bytes")
             if status != 0:
@@ -554,14 +568,15 @@ class GatewayDecompressVerify(GatewayOperator):
                 want = bytes.fromhex(want)
             if want is not None and bytes(want) != digest:
                 raise ChecksumMismatchException(f"chunk {chunk.chunk_id}: md5 {digest.hex()} != expected {bytes(want).hex()}")
-            path = self.chunk_store.get_chunk_file_path(chunk.chunk_id)
-            tmp = path.with_name(path.name + ".part")
-            with open(tmp, "wb") as f:
-                f.write(data)
-            os.replace(tmp, path)
+            if not in_place:
+                path = self.chunk_store.get_chunk_file_path(chunk.chunk_id)
+                tmp = path.with_name(path.name + ".part")
+                with open(tmp, "wb") as f:
+                    f.write(data)
+                os.replace(tmp, path)
             chunk.md5_hash = digest  # lets the upload step send Content-MD5 (gateway_operator.py:640)
             self._seen.pop(chunk.chunk_id, None)
-            if self.remove_frames:
+            if self.remove_frames and not in_place:
                 self.chunk_store.get_compressed_file_path(chunk.chunk_id).unlink(missing_ok=True)
             ok[i] = True
         return ok

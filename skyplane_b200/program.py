@@ -43,7 +43,9 @@ def _compress_hash(op: Dict, kw: Dict) -> GatewayOperator:
 
 
 def _decompress_verify(op: Dict, kw: Dict) -> GatewayOperator:
-    return GatewayDecompressVerify(**kw, n_processes=op.get("num_gpus", 1), n_gpus=op.get("num_gpus"))
+    # "compress" as on compress_hash and the reference's send / receive nodes: false when the sender's is false
+    return GatewayDecompressVerify(**kw, n_processes=op.get("num_gpus", 1), n_gpus=op.get("num_gpus"),
+                                   use_compression=op.get("compress", True))
 
 
 def _receive(op: Dict, kw: Dict) -> GatewayOperator:

@@ -255,36 +255,50 @@ class ChunkStage:
         return out
 
     # ------------------------------------------------------------------ receiver side
-    def decode(self, frames: Sequence[BytesLike], raw_lens: Sequence[int], encrypted: bool = False):
+    def decode(self, frames: Sequence[BytesLike], raw_lens: Sequence[int], encrypted: bool = False, compressed: bool = True):
         """Decode LZ4 frames and digest the decoded bytes (gateway_receiver.py:195-201 + the missing hash check);
         encrypted=True: the payloads are SecretBox messages, opened on the device first (gateway_receiver.py:191-193).
-        -> list of (data: bytes | None, md5: bytes, status: int); data is None when status != 0."""
+        compressed=False: the sender ran with `compress: false`, so the payloads (or what their boxes hold) are the chunks
+        themselves (``is_compressed = False``, gateway_receiver.py:195): they are digested, and checked against raw_lens.
+        -> list of (data: bytes | None, md5: bytes, status: int); data is None when status != 0 -- and for a payload that is
+        the chunk already (compressed=False without encryption), which the caller holds."""
+        if len(frames) != len(raw_lens):
+            raise ValueError(f"{len(frames)} payloads but {len(raw_lens)} raw lengths")
         out = []
         i = 0
         if self._free is None or not self._free:
             raise native.SkyChunkError(native.SKY_E_BUSY, "collect() pending batches before decode()")
-        slot = self._free[-1]  # its pinned buffers are idle: frames are staged in `out`, decoded bytes land in `inp`
+        slot = self._free[-1]  # its pinned buffers are idle: frames and boxes are staged in `out`, decoded or opened bytes land
+        #                        in `inp`; a payload that is the chunk itself is staged in `inp` and nothing comes back
+        digest_only = not compressed and not encrypted
+        flags = (0 if compressed else native.F_MD5) | (native.F_E2EE if encrypted else 0)
         while i < len(frames):
             f_off, o_off, fp, op = [], [], 0, 0
             j = i
             while j < len(frames) and j - i < self.max_chunks:
                 fl, rl = memoryview(frames[j]).nbytes, raw_lens[j]
-                if fp + native.round16(fl) > slot.out.nbytes or op + native.round16(rl) > slot.inp.nbytes:
-                    break
-                slot.out.view[fp : fp + fl] = memoryview(frames[j]).cast("B")
+                if digest_only:
+                    if fp + native.round16(fl) > slot.inp.nbytes:
+                        break
+                    slot.inp.view[fp : fp + fl] = memoryview(frames[j]).cast("B")
+                else:
+                    if fp + native.round16(fl) > slot.out.nbytes or op + native.round16(rl) > slot.inp.nbytes:
+                        break
+                    slot.out.view[fp : fp + fl] = memoryview(frames[j]).cast("B")
+                    o_off.append(op)
+                    op += native.round16(rl)
                 f_off.append(fp)
-                o_off.append(op)
                 fp += native.round16(fl)
-                op += native.round16(rl)
                 j += 1
             if j == i:
-                raise native.SkyChunkError(native.SKY_E_CAPACITY, "frame exceeds the stage's staging buffers")
+                raise native.SkyChunkError(native.SKY_E_CAPACITY, "payload exceeds the stage's staging buffers")
             lens = [memoryview(frames[k]).nbytes for k in range(i, j)]
             raws = list(raw_lens[i:j])
-            st, dg, self.last_kernel_ms = self.ctx.decode([slot.out.addr + o for o in f_off], lens, [slot.inp.addr + o for o in o_off], raws,
-                                                          native.F_E2EE if encrypted else 0)
+            src = slot.inp.addr if digest_only else slot.out.addr
+            st, dg, self.last_kernel_ms = self.ctx.decode([src + o for o in f_off], lens,
+                                                          None if digest_only else [slot.inp.addr + o for o in o_off], raws, flags)
             for k in range(j - i):
-                data = bytes(slot.inp.view[o_off[k] : o_off[k] + raws[k]]) if st[k] == 0 else None
+                data = bytes(slot.inp.view[o_off[k] : o_off[k] + raws[k]]) if st[k] == 0 and not digest_only else None
                 out.append((data, dg[k], st[k]))
             i = j
         return out

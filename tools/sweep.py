@@ -11,7 +11,10 @@ input: independent or linked blocks, without checksums or with block and content
 --ref-ratio adds the reference's ratio (liblz4 level 0, linked blocks) on the distinct chunks; --liblz4-level9 times liblz4
 level 9 with independent blocks on all of the host's cores (the rate the reference's sender would get from that level).
 --verify also times SKY_F_VERIFY's check (sky_verify_device, check only) of every frame set right after it is made, in the
-same iterations: kernel_ms (frames), verify_ms (their check) and kernel_plus_verify_ms; every status must be 0."""
+same iterations: kernel_ms (frames), verify_ms (their check) and kernel_plus_verify_ms; every status must be 0.
+--decode-raw [--e2ee] is a sweep of its own, on the host path: Context.decode of `compress: false` payloads (the chunks
+themselves, or with --e2ee their SecretBoxes) beside the LZ4 receive of the same chunks (their frames, or the frames' boxes),
+alternated call by call: kernel_ms (device events) and call_ms (host clock around the synchronous call, copies included)."""
 import argparse
 import json
 import multiprocessing as mp
@@ -98,6 +101,69 @@ def liblz4_frames(d_in, stride, n, chunk_bytes, d_out, dst_off, linked, checksum
     return lens
 
 
+def decode_raw_sweep(total_mib, chunk_mib, iters, e2ee):
+    """Time sky_decode on raw payloads and on LZ4 frames of the same random chunks (host buffers, pinned), alternated.
+    The sender on the same ctx makes the payloads of 16 distinct chunks; the n payloads of a call cycle through them."""
+    import hashlib
+    import subprocess
+
+    chunk_bytes = int(chunk_mib * (1 << 20))
+    n = max(1, (total_mib << 20) // chunk_bytes)
+    stride, n_pool = native.round16(chunk_bytes), min(16, n)
+    room = native.round16(native.frame_bound(chunk_bytes) + native.BOX_OVERHEAD)
+    src, frames, boxes, dst = (native.PinnedBuffer(k) for k in (n_pool * stride, n_pool * room, n_pool * room, n * stride))
+    for i in range(n_pool):
+        src.view[i * stride : i * stride + chunk_bytes] = synth.random_chunk(4000 + i, chunk_bytes)
+    want = [hashlib.md5(src.view[i * stride : i * stride + chunk_bytes]).digest() for i in range(n_pool)]
+    ctx = native.Context(0, n * stride, n, 1)
+    key = bytes(range(32))
+    ctx.set_e2ee_key(key)
+    seal = native.F_E2EE if e2ee else 0
+    src_addrs, lens = [src.addr + i * stride for i in range(n_pool)], [chunk_bytes] * n_pool
+    nonces = os.urandom(24 * n_pool) if e2ee else None
+    frame_lens, dg, _ = ctx.wait(ctx.submit(src_addrs, lens, [frames.addr + i * room for i in range(n_pool)], [room] * n_pool,
+                                            native.F_LZ4 | native.F_MD5 | seal, nonces))
+    assert dg == want
+    if e2ee:
+        box_lens, dg, _ = ctx.wait(ctx.submit(src_addrs, lens, [boxes.addr + i * room for i in range(n_pool)], [room] * n_pool,
+                                              native.F_MD5 | seal, nonces))
+        assert dg == want
+    cyc = [i % n_pool for i in range(n)]
+    dst_addrs = [dst.addr + i * stride for i in range(n)]
+    legs = {"lz4": ([frames.addr + k * room for k in cyc], [frame_lens[k] for k in cyc], dst_addrs, seal),
+            "raw": ([boxes.addr + k * room for k in cyc], [box_lens[k] for k in cyc], dst_addrs, native.F_MD5 | seal) if e2ee else
+                   ([src.addr + k * stride for k in cyc], [chunk_bytes] * n, None, native.F_MD5)}
+    kms, wall, ok = {k: [] for k in legs}, {k: [] for k in legs}, {k: True for k in legs}
+    for it in range(iters + 1):
+        for name, (addrs, plens, out, flags) in legs.items():
+            t = time.perf_counter()
+            st, dg, k = ctx.decode(addrs, plens, out, [chunk_bytes] * n, flags)
+            w = (time.perf_counter() - t) * 1e3
+            ok[name] = ok[name] and all(x == 0 for x in st) and dg == [want[k] for k in cyc]
+            if out is not None:
+                ok[name] = ok[name] and all(dst.view[i * stride : i * stride + chunk_bytes] == src.view[k * stride : k * stride + chunk_bytes]
+                                            for i, k in list(enumerate(cyc))[:: max(1, n // 8)])
+            if it:
+                kms[name].append(k)
+                wall[name].append(w)
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+        gpu = q.stdout.strip() or torch.cuda.get_device_name(0)
+    except OSError:
+        gpu = torch.cuda.get_device_name(0)
+    for name in legs:
+        k = statistics.median(kms[name])
+        print(json.dumps({"workload": "random", "chunk_mib": float(chunk_mib), "chunks": n, "distinct_chunks": n_pool, "path": "Context.decode (host buffers)",
+                          "payload": ("box of " if e2ee else "") + ("lz4 frame" if name == "lz4" else "raw chunk"), "launches_per_call": {
+                              "lz4": 5 if e2ee else 2, "raw": 4 if e2ee else 1}[name], "kernel_ms": k, "kernel_ms_min": min(kms[name]),
+                          "kernel_ms_max": max(kms[name]), "kernel_ms_covers": "index + decode + MD5 (the box open is outside it)" if name == "lz4"
+                          else ("open + MD5" if e2ee else "MD5"), "call_ms": statistics.median(wall[name]), "raw_output_gbs": n * chunk_bytes / k / 1e6,
+                          "iters": iters, "all_ok": ok[name], "gpu": gpu}), flush=True)
+    ctx.close()
+    for b in (src, frames, boxes, dst):
+        b.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--total-mib", type=int, default=2048)
@@ -111,7 +177,12 @@ def main():
     ap.add_argument("--ref-ratio", action="store_true", help="also the reference's ratio on the distinct chunks (CPU)")
     ap.add_argument("--liblz4-level9", action="store_true", help="also liblz4 level 9 on all host cores (CPU)")
     ap.add_argument("--verify", action="store_true", help="also time the frame check (SKY_F_VERIFY) of each flag set's frames")
+    ap.add_argument("--decode-raw", action="store_true", help="only: Context.decode of raw (`compress: false`) payloads beside the LZ4 "
+                    "receive of the same random chunks, alternated (--total-mib, the first of --sizes-mib, --iters)")
+    ap.add_argument("--e2ee", action="store_true", help="with --decode-raw: the payloads are SecretBoxes")
     a = ap.parse_args()
+    if a.decode_raw:
+        return decode_raw_sweep(a.total_mib, float(a.sizes_mib.split(",")[0]), a.iters, a.e2ee)
     dev = torch.device("cuda", 0)
     FL = {"lz4": native.F_LZ4, "md5": native.F_MD5, "both": 0, "hc": native.F_HC, "hc-lz4": native.F_HC | native.F_LZ4,
           "checksum": native.F_CHECKSUM, "hc-checksum": native.F_HC | native.F_CHECKSUM}
