@@ -23,6 +23,17 @@
  *   emit    = the block's sequences are the segments' sequences in order; literals a segment leaves behind its last match
  *             (or a whole segment without a match) are carried into the next sequence.  Standard LZ4 block format.
  *             A block whose compressed size would exceed L-1 is stored raw (return 0), as LZ4F_makeBlock does.
+ *   linked  = (study mode, tile_compress_block_linked; the kernel does not implement it) blocks j >= 1 of a chunk may
+ *             match into the previous 64 KiB window, FLG B.Indep clear (for chunks of more than one block, see
+ *             tools/tile_model.py).  The table starts seeded from that window instead of empty: its positions
+ *             65536 - seed .. 65531 inserted in order, last writer wins (what sequential insertion leaves behind),
+ *             each as (pos16 | tag16) with pos16 relative to the previous block.  A probe's candidate offset is
+ *             (p - pos16) mod 65536: an entry above p is in the previous window at offset p + 65536 - pos16, one below p
+ *             is in this block (a seeded entry below p is read as a position of this block: the parse verifies every
+ *             candidate, so such a stale entry only costs a probe).  Offset 0 is no hit.  Nothing else changes: the
+ *             parse verifies and extends against the chunk's source bytes (backward extension may cross the block
+ *             start), and block j depends on source bytes only, never on block j-1's compressed output.  Block 0 of a
+ *             chunk is the independent block.
  *
  * Build: gcc -O2 -shared -fPIC -o tools/bin/liblz4tile.so tools/lz4_tile_model.c
  */
@@ -68,10 +79,17 @@ typedef struct { uint64_t probes, hits, accepted, segments; } tile_stats;
 static tile_stats g_stats;
 void tile_model_stats(tile_stats *s, int reset) { *s = g_stats; if (reset) memset(&g_stats, 0, sizeof g_stats); }
 
-/* returns compressed size, or 0 if the block does not shrink (store raw); out capacity >= L + 2048 */
-uint32_t tile_compress_block(const uint8_t *src, uint32_t L, uint8_t *out, const tile_opts *o) {
+/* returns compressed size, or 0 if the block does not shrink (store raw); out capacity >= L + 2048.
+   prefix = bytes of the previous window readable before src (0: an independent block; linked: 65536 for blocks j >= 1),
+   seed = how many of its last positions seed the table (linked only). */
+static uint32_t compress_block(const uint8_t *src, uint32_t L, uint8_t *out, const tile_opts *o, uint32_t prefix, uint32_t seed) {
     const uint32_t S = (uint32_t)o->seg_slots, limit = L - 1;
     uint32_t *tab = calloc((size_t)o->entries, 4);  /* pos | tag << 16 ; 0 = (pos 0, tag 0) = "empty" */
+    if (prefix)  /* linked: the previous window's positions q (hash inside the window), in order, the last one staying */
+        for (uint32_t q = prefix - seed; q + 5 <= prefix; q++) {
+            const uint32_t hf = hash5(src - prefix + q);
+            tab[hidx(hf, o)] = q | (htag(hf) << 16);
+        }
     uint16_t *off = malloc(2 * S);
     uint8_t *hit = malloc(S);
     uint32_t anchor = 0 /* start of the literals not yet emitted */, op = 0, result = 0;
@@ -93,7 +111,9 @@ uint32_t tile_compress_block(const uint8_t *src, uint32_t L, uint8_t *out, const
                     const uint32_t e = tab[hidx(hf, o)], epos = e & 0xffffu;
                     ghf[i - g] = hf;
                     g_stats.probes++;
-                    if ((e >> 16) == htag(hf) && epos < p) { hit[i] = 1; off[i] = (uint16_t)(p - epos); }
+                    if (prefix) {  /* linked: offset (p - pos16) mod 65536, 0 = no hit */
+                        if ((e >> 16) == htag(hf) && ((p - epos) & 0xffffu)) { hit[i] = 1; off[i] = (uint16_t)(p - epos); }
+                    } else if ((e >> 16) == htag(hf) && epos < p) { hit[i] = 1; off[i] = (uint16_t)(p - epos); }
                     if (o->group_lag) {  /* an equal hash 3, 4 or 8 slots back in the group is the nearer candidate */
                         for (uint32_t d = 1; d <= i - g; d++)
                             if ((((uint32_t)o->near_mask >> (d - 1)) & 1u) && ghf[i - g - d] == hf) { hit[i] = 1; off[i] = (uint16_t)(d << slog); break; }
@@ -115,20 +135,20 @@ uint32_t tile_compress_block(const uint8_t *src, uint32_t L, uint8_t *out, const
                 if (!hit[i]) continue;
                 uint32_t pos = seg_pos + (i << slog);
                 if (pos < cur || pos >= mlim) continue;
-                uint32_t cand = pos - off[i];
+                int64_t cand = (int64_t)pos - off[i];  /* < 0: in the previous window (linked) */
                 const uint32_t maxlen = mlim - pos;
                 uint32_t mlen = 0;
                 while (mlen < maxlen && src[pos + mlen] == src[cand + mlen]) mlen++;
                 if (mlen < MINMATCH) continue;
                 if (o->back_ext) {
                     uint32_t room = pos - lanchor;
-                    if (cand < room) room = cand;
+                    if (cand + prefix < room) room = (uint32_t)(cand + prefix);
                     if (room > 8) room = 8;
                     uint32_t b = 0;
                     while (b < room && src[pos - 1 - b] == src[cand - 1 - b]) b++;
                     pos -= b; cand -= b; mlen += b;
                 }
-                op = emit(out, op, src, anchor, pos - anchor, mlen, pos - cand);
+                op = emit(out, op, src, anchor, pos - anchor, mlen, (uint32_t)(pos - cand));
                 anchor = cur = lanchor = pos + mlen;
                 g_stats.accepted++;
                 if (op > L + 1024) goto done;  /* (model only) hopeless and about to overrun the caller's buffer */
@@ -147,4 +167,13 @@ uint32_t tile_compress_block(const uint8_t *src, uint32_t L, uint8_t *out, const
 done:
     free(tab); free(off); free(hit);
     return result;
+}
+
+uint32_t tile_compress_block(const uint8_t *src, uint32_t L, uint8_t *out, const tile_opts *o) {
+    return compress_block(src, L, out, o, 0, 0);
+}
+
+/* block j >= 1 of a linked chunk: src[-65536 .. -1] is block j-1; seed = its last positions that seed the table */
+uint32_t tile_compress_block_linked(const uint8_t *src, uint32_t L, uint8_t *out, const tile_opts *o, uint32_t seed) {
+    return compress_block(src, L, out, o, 65536, seed);
 }

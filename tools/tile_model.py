@@ -35,6 +35,8 @@ def lib():
         _lib = ctypes.CDLL(str(_SO))
         _lib.tile_compress_block.argtypes = [ctypes.c_char_p, ctypes.c_uint32, ctypes.c_char_p, ctypes.POINTER(Opts)]
         _lib.tile_compress_block.restype = ctypes.c_uint32
+        _lib.tile_compress_block_linked.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_char_p, ctypes.POINTER(Opts), ctypes.c_uint32]
+        _lib.tile_compress_block_linked.restype = ctypes.c_uint32
     return _lib
 
 
@@ -56,26 +58,36 @@ def _xxh32_small(b: bytes) -> int:  # XXH32, seed 0, inputs < 16 bytes (the fram
     return h ^ (h >> 16)
 
 
-def blocks(data: bytes, o: Opts):
-    """-> list of (compressed size or 0 when stored raw, block bytes as they appear in the frame)."""
+SEED = 65536  # linked: positions of the previous window that seed a block's table (the rule DESIGN §4.2 measures)
+
+
+def blocks(data: bytes, o: Opts, linked: bool = False, seed: int = SEED):
+    """-> list of (compressed size or 0 when stored raw, block bytes as they appear in the frame).  linked:
+    blocks after the first may match into the previous 64 KiB window, from a table seeded with its last `seed` positions."""
     L = lib()
     buf = ctypes.create_string_buffer(65536 + 4096)
+    src = ctypes.create_string_buffer(bytes(data), len(data)) if linked else None
     out = []
     for pos in range(0, len(data), 65536):
         blk = data[pos:pos + 65536]
-        c = L.tile_compress_block(blk, len(blk), buf, ctypes.byref(o))
+        if linked and pos:
+            c = L.tile_compress_block_linked(ctypes.addressof(src) + pos, len(blk), buf, ctypes.byref(o), seed)
+        else:
+            c = L.tile_compress_block(blk, len(blk), buf, ctypes.byref(o))
         out.append((c, buf.raw[:c] if c else blk))
     return out
 
 
-def assemble(n: int, blks, block_checksum: bool = False) -> bytes:
+def assemble(n: int, blks, block_checksum: bool = False, linked: bool = False) -> bytes:
     """The stage's frame around an n-byte chunk's blocks [(compressed size or 0 when stored raw, block bytes)];
-    block_checksum (SKY_F_BLOCK_CHECKSUM): FLG's B.Checksum bit, and u32le XXH32 of every block's bytes behind them."""
-    flg = 0x10 if block_checksum else 0
+    block_checksum (SKY_F_BLOCK_CHECKSUM): FLG's B.Checksum bit, and u32le XXH32 of every block's bytes behind them;
+    linked (linked-block mode): FLG's B.Indep bit clear when the chunk has more than one block -- liblz4 declares a frame
+    of at most one block independent whatever blockMode asks for, and so does this header."""
+    flg = (0x10 if block_checksum else 0) | (0 if linked and n > 65536 else 0x20)
     if not n:
-        d = bytes([0x60 | flg, 0x40])
+        d = bytes([0x40 | flg, 0x40])
         return bytes([0x04, 0x22, 0x4D, 0x18]) + d + bytes([(_xxh32_small(d) >> 8) & 0xFF]) + bytes(4)
-    d = bytes([0x68 | flg, 0x40]) + n.to_bytes(8, "little")
+    d = bytes([0x48 | flg, 0x40]) + n.to_bytes(8, "little")
     fr = bytearray(bytes([0x04, 0x22, 0x4D, 0x18]) + d + bytes([(_xxh32_small(d) >> 8) & 0xFF]))
     for c, b in blks:
         fr += (c if c else (len(b) | 0x80000000)).to_bytes(4, "little") + b
@@ -91,5 +103,5 @@ def xxh32(b: bytes) -> int:
     return oracle.xxh32(b)
 
 
-def frame(data: bytes, o: Opts | None = None, block_checksum: bool = False) -> bytes:
-    return assemble(len(data), blocks(data, o or kernel_opts()), block_checksum)
+def frame(data: bytes, o: Opts | None = None, block_checksum: bool = False, linked: bool = False) -> bytes:
+    return assemble(len(data), blocks(data, o or kernel_opts(), linked), block_checksum, linked)
