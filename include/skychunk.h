@@ -100,6 +100,16 @@ extern "C" {
  * (sky_verify_device runs the same check over frames in HBM).  Three more launches per batch.  It sits outside the
  * SKY_F_HC_LEVEL field. */
 #define SKY_F_VERIFY 4096u
+/* linked blocks (python-lz4's block_linked, liblz4's blockMode = linked), with SKY_F_HC / SKY_F_HC_LEVEL only (sky_submit,
+ * sky_process_device, sky_verify_device): a match may reach up to 65535 bytes back, across its block's start into the
+ * previous block of the chunk, which on text saves 9-17 % of the high-ratio mode's bytes.  FLG clears B.Indep (0x48,
+ * 0x4C / 0x58 / 0x5C with the checksum flags) for a chunk of more than one block; a chunk of at most one block keeps the
+ * independent FLG, as liblz4 writes it.  Every block is still made from the chunk's source bytes alone, so blocks compress
+ * in parallel.  The receiver (sky_decode, lz4.frame.decompress) decodes a linked frame's blocks one after the other within
+ * the chunk.  Without SKY_F_HC, or with SKY_F_MD5 alone, it is SKY_E_INVALID: the fast compressor has no linked mode, since its
+ * parse would trail the reference's ratio even with the window.  sky_decode does not take it: a frame states its own block
+ * mode. */
+#define SKY_F_LINKED 8192u
 
 typedef struct sky_ctx sky_ctx;
 

@@ -23,23 +23,31 @@ __device__ __forceinline__ uint32_t frame_header_bytes(uint64_t n) { return n ? 
 __device__ __forceinline__ uint32_t frame_flg(uint32_t flags) {
     return ((flags & SKY_F_CHECKSUM) ? 0x04u : 0u) | ((flags & SKY_F_BLOCK_CHECKSUM) ? 0x10u : 0u);
 }
+// FLG's B.Indep (0x20) for an n-byte chunk: set, unless SKY_F_LINKED links the blocks of a chunk of more than one block
+// (liblz4 declares a frame of at most one block independent whatever blockMode asks for).  kLinkable: the caller may see
+// SKY_F_LINKED (the linked compressor and frame check); every other caller writes independent frames only.
+template <bool kLinkable>
+__device__ __forceinline__ uint32_t frame_indep(uint32_t flags, uint64_t n) {
+    return (kLinkable && (flags & SKY_F_LINKED) && n > kBlock) ? 0u : 0x20u;
+}
 
 __device__ __forceinline__ void st_u32le(uint8_t *p, uint32_t v) {
     p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24);
 }
 
 // Single thread: writes the final frame header of an n-byte chunk made with the batch's `flags`; returns its size.
+template <bool kLinkable = false>
 __device__ __forceinline__ uint32_t write_frame_header(uint8_t *dst, uint64_t n, uint32_t flags) {
     uint8_t d[10];
     d[1] = 0x40;  // BD: 64 KiB blocks
     st_u32le(dst, 0x184D2204u);  // magic
     if (n == 0) {
-        d[0] = (uint8_t)(0x60u | frame_flg(flags));  // v01 | B.Indep
+        d[0] = (uint8_t)(0x40u | frame_indep<kLinkable>(flags, n) | frame_flg(flags));  // v01 | B.Indep
         dst[4] = d[0]; dst[5] = d[1];
         dst[6] = (uint8_t)(xxh32_small(d, 2) >> 8);
         return 7;
     }
-    d[0] = (uint8_t)(0x68u | frame_flg(flags));  // v01 | B.Indep | C.Size
+    d[0] = (uint8_t)(0x48u | frame_indep<kLinkable>(flags, n) | frame_flg(flags));  // v01 | B.Indep | C.Size
 #pragma unroll
     for (int i = 0; i < 8; i++) d[2 + i] = (uint8_t)(n >> (8 * i));
 #pragma unroll
@@ -106,7 +114,8 @@ __device__ __forceinline__ void st_release32(uint32_t *p, uint32_t v) {
 }
 
 // One thread: claim the next block that has LZ4 work (empty chunks are finished on the spot) and describe it to the CTA.
-// Block 0's claim writes the frame header.
+// Block 0's claim writes the frame header (kLinkable: write_frame_header's).
+template <bool kLinkable = false>
 __device__ __forceinline__ void claim_block(const Params &p, BlockDesc *d) {
     const uint32_t total = p.rows * p.n_chunks;
     // read per claim: hoisted out of the kernel's block loop, the FLG bits would hold a register there (sky_fused_kernel spills)
@@ -122,7 +131,7 @@ __device__ __forceinline__ void claim_block(const Params &p, BlockDesc *d) {
         const ChunkDesc cd = p.chunks[c];
         if (cd.nblk == 0) {
             if (j == 0) {  // empty chunk: 7-byte header + EndMark
-                const uint32_t h = write_frame_header(cd.dst, 0, flags);
+                const uint32_t h = write_frame_header<kLinkable>(cd.dst, 0, flags);
                 st_u32le(cd.dst + h, 0);
                 p.out_len[c] = h + 4;
             }
@@ -137,7 +146,7 @@ __device__ __forceinline__ void claim_block(const Params &p, BlockDesc *d) {
         d->L = (uint32_t)min((uint64_t)kBlock, cd.len - boff);
         d->last = (j + 1 == cd.nblk);
         d->valid = 1;
-        if (j == 0) write_frame_header(cd.dst, cd.len, flags);
+        if (j == 0) write_frame_header<kLinkable>(cd.dst, cd.len, flags);
         return;
     }
 }

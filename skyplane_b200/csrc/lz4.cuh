@@ -294,14 +294,14 @@ __device__ __forceinline__ uint32_t load32s(uint32_t in_s, uint32_t pos) {
     return __funnelshift_r(lds32(a), lds32(a + 4), (pos & 3u) * 8u);
 }
 
-// ---- cooperative forward extension in shared memory: all lanes compare 4 bytes each per round
-__device__ __forceinline__ uint32_t extend_coop_s(uint32_t in32, uint32_t mpos, uint32_t mcand, uint32_t mlen, uint32_t maxlen,
-                                                  unsigned lane) {
+// ---- cooperative forward extension: all lanes compare 4 bytes each per round; load4(pos) reads the 4 bytes at pos
+template <class Load4>
+__device__ __forceinline__ uint32_t extend_coop(Load4 load4, uint32_t mpos, uint32_t mcand, uint32_t mlen, uint32_t maxlen, unsigned lane) {
     for (;;) {
         const uint32_t o = mlen + lane * 4;
         uint32_t cnt = 0;
         if (o < maxlen) {
-            const uint32_t x = load32s(in32, mpos + o) ^ load32s(in32, mcand + o);
+            const uint32_t x = load4(mpos + o) ^ load4(mcand + o);
             cnt = x ? (uint32_t)(__ffs(x) - 1) >> 3 : 4u;
             cnt = min(cnt, maxlen - o);
         }
@@ -313,6 +313,11 @@ __device__ __forceinline__ uint32_t extend_coop_s(uint32_t in32, uint32_t mpos, 
         const int f = __ffs(~fullm) - 1;
         return mlen + 4 * f + __shfl_sync(kFull, cnt, f);
     }
+}
+// ... in shared memory
+__device__ __forceinline__ uint32_t extend_coop_s(uint32_t in32, uint32_t mpos, uint32_t mcand, uint32_t mlen, uint32_t maxlen,
+                                                  unsigned lane) {
+    return extend_coop([in32](uint32_t pos) { return load32s(in32, pos); }, mpos, mcand, mlen, maxlen, lane);
 }
 
 // ---- emission of up to 32 recorded sequences, one per lane ------------------------------------------

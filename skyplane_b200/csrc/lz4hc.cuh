@@ -18,6 +18,18 @@
 //            emitted 32 at a time (flush_seqs) into the scratch; the block is stored raw when that is not smaller;
 //   place  : the OFF chain gives the block's frame offset (place_block), and all warps copy it there.
 // Claim, load, placement and write-out are frame.cuh's, shared with sky_fused_kernel.
+//
+// Linked blocks (SKY_F_LINKED, sky_hc_linked{,_bc}_kernel): block j >= 1 of a chunk also sees the chunk's 64 KiB before it
+// (the twin's hc_compress_block_linked).  Shared memory has no room for that window, so it stays where it is:
+//   window bytes : read from the chunk in global memory (d.src - 65536, L2-resident) by load32x / load8x, which read shared
+//                  memory for a position in the block and global memory for one before it;
+//   window chains: u16 distances of the window's positions in the CTA's scratch (kHcHistOff, 128 KiB more per CTA);
+//   head         : still u16.  A bitmap in shared memory (kHcBitOff, 2 KiB) marks the hashes whose head this block has
+//                  written; an unmarked non-zero head is a window position, stored as its index in the previous block.
+// Chains: all warps hash the window into the chain array (free until the block's own chains), then warp 0 inserts the
+// window's positions 1 .. 65535 and then the block's, in order: exact sequential insertion.  (Window position 0 lies
+// 65536 bytes before every block position, so leaving it out changes no walk.)  A link longer than 65535 bytes is stored
+// as "none"; a walk stops at the first candidate more than 65535 bytes back, as the twin's does.
 #pragma once
 #include "frame.cuh"
 
@@ -47,24 +59,42 @@ constexpr uint32_t kHcHeadOff = kHcChainOff + 2 * kBlock;         // u16 per has
 constexpr uint32_t kHcCtlOff = kHcHeadOff + (2u << kHcHashBits);
 constexpr uint32_t kHcSmemBytes = kHcCtlOff + (uint32_t)sizeof(HcCtl);
 static_assert(kHcSmemBytes <= 232448, "one HC CTA per SM: at most 227 KiB of shared memory");
-// per-CTA scratch in global memory: lengths (u8), offsets (u16) and the compressed block
+constexpr uint32_t kHcBitOff = (kHcSmemBytes + 15u) & ~15u;                // linked: 1 bit per hash, "head written in this block"
+constexpr uint32_t kHcLinkedSmemBytes = kHcBitOff + (1u << kHcHashBits) / 8;
+static_assert(kHcLinkedSmemBytes <= 232448, "one linked HC CTA per SM: at most 227 KiB of shared memory");
+// per-CTA scratch in global memory: lengths (u8), offsets (u16) and the compressed block; linked, the window's chains (u16)
 constexpr uint32_t kHcLenOff = 0, kHcOffOff = kBlock, kHcOutOff = 3 * kBlock;
 constexpr uint32_t kHcScratchBytes = 4 * kBlock + 2048;
+constexpr uint32_t kHcHistOff = kHcScratchBytes, kHcLinkedScratchBytes = kHcHistOff + 2 * kBlock;
+constexpr uint32_t kHcWindow = 65535;  // the largest offset
+
+// Linked: the source bytes at position x of the block (x < 0: the previous block's, x >= -65536), from shared memory
+// (in_s) in the block and from the chunk in global memory (src = the block's start, 16-byte aligned) before it.
+__device__ __forceinline__ uint32_t load32x(uint32_t in_s, const uint8_t *src, int32_t x) {
+    if (x >= 0) return load32s(in_s, (uint32_t)x);
+    const uint32_t *w = reinterpret_cast<const uint32_t *>(src + (x & ~3));
+    return __funnelshift_r(__ldg(w), __ldg(w + 1), (uint32_t)(x & 3) * 8u);
+}
+__device__ __forceinline__ uint32_t load8x(uint32_t in_s, const uint8_t *src, int32_t x) {
+    return x >= 0 ? lds8(in_s + (uint32_t)x) : (uint32_t)__ldg(src + x);
+}
 
 // kHcDepth: chain candidates walked per position, hc_depth(level).  kBlkChk (SKY_F_BLOCK_CHECKSUM): every block gets its
 // checksum (block_checksum), hashed from the frame by warp 1 during the next block's chain step, which only warp 0 works
-// on (or before the CTA exits).
-template <uint32_t kHcDepth, bool kBlkChk>
+// on (or before the CTA exits).  kLinked (SKY_F_LINKED): blocks after a chunk's first match into its previous 64 KiB.
+template <uint32_t kHcDepth, bool kBlkChk, bool kLinked = false>
 __device__ __forceinline__ void hc_body(const Params &p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     uint8_t *in = smem + kHcInOff;
     HcCtl *ctl = reinterpret_cast<HcCtl *>(smem + kHcCtlOff);
     const uint32_t in_s = smem_u32(in), chain_s = smem_u32(smem + kHcChainOff), head_s = smem_u32(smem + kHcHeadOff);
-    uint8_t *scr = p.scratch + (size_t)blockIdx.x * kHcScratchBytes;
+    uint8_t *scr = p.scratch + (size_t)blockIdx.x * (kLinked ? kHcLinkedScratchBytes : kHcScratchBytes);
     uint8_t *g_len = scr + kHcLenOff;
     uint16_t *g_off = reinterpret_cast<uint16_t *>(scr + kHcOffOff);
     uint8_t *cout = scr + kHcOutOff;
+    uint16_t *g_hist = reinterpret_cast<uint16_t *>(scr + kHcHistOff);  // linked: chain distance of window position i
+    const uint32_t bit_s = smem_u32(smem + kHcBitOff);
     if (tid == 0) {
         mbar_init(&ctl->in_full, 1);
         if constexpr (kBlkChk) ctl->pend.data = nullptr;
@@ -73,7 +103,7 @@ __device__ __forceinline__ void hc_body(const Params &p) {
     __syncthreads();
 
     for (uint32_t in_phase = 0;; in_phase ^= 1) {
-        if (tid == 0) claim_block(p, &ctl->desc);
+        if (tid == 0) claim_block<kLinked>(p, &ctl->desc);
         __syncthreads();  // (also: every warp is done with the previous block)
         const BlockDesc d = ctl->desc;
         if (!d.valid) {
@@ -86,12 +116,41 @@ __device__ __forceinline__ void hc_body(const Params &p) {
         if (tid == 0) load_block(in, d.src, L, &ctl->in_full);
         uint4 *h4 = reinterpret_cast<uint4 *>(smem + kHcHeadOff);
         for (uint32_t k = tid; k < (2u << kHcHashBits) / 16; k += kHcThreads) h4[k] = make_uint4(0, 0, 0, 0);
+        const bool window = kLinked && d.j > 0 && L >= kMfLimit + 1;  // linked: this block sees the previous one
+        if constexpr (kLinked) {
+            uint4 *b4 = reinterpret_cast<uint4 *>(smem + kHcBitOff);
+            for (uint32_t k = tid; k < (1u << kHcHashBits) / 128; k += kHcThreads) b4[k] = make_uint4(0, 0, 0, 0);
+            if (window) {  // the window's hashes, into the chain array: position i of the previous block at i * 2
+                const uint8_t *prev = d.src - kBlock;
+                for (uint32_t i = tid; i < kBlock; i += kHcThreads) {
+                    const uint32_t *w = reinterpret_cast<const uint32_t *>(prev + (i & ~3u));
+                    const uint32_t v = __funnelshift_r(__ldg(w), __ldg(w + 1), (i & 3u) * 8u);
+                    sts16(chain_s + i * 2u, (v * 2654435761u) >> (32 - kHcHashBits));
+                }
+            }
+        }
         mbar_wait(&ctl->in_full, in_phase);
         __syncthreads();  // the head table is clear
 
         const uint32_t mflimit = L - kMfLimit, matchlimit = L - kLastLiterals;  // (meaningful when L > kMfLimit)
         const bool has_matches = L >= kMfLimit + 1;
         // ---------------------------------------------------------------- chains (warp 0)
+        if (window && warp == 0) {  // the window's positions 1 .. 65535 first; head = the position's index, 1 .. 65535
+            for (uint32_t base = 0; base < kBlock; base += 32) {
+                const uint32_t i = base + lane;
+                const bool valid = i != 0;
+                const uint32_t h = valid ? lds16(chain_s + i * 2u) : 0x80000000u;
+                const unsigned same = __match_any_sync(kFull, h);
+                const unsigned lower = same & ((1u << lane) - 1u);
+                const uint32_t prev = lower ? base + bfind(lower) : (valid ? lds16(head_s + h * 2u) : 0u);
+                __syncwarp();
+                if (valid) {
+                    if ((same >> lane) == 1u) sts16(head_s + h * 2u, i);
+                    g_hist[i] = (uint16_t)(prev ? i - prev : 0u);
+                }
+                __syncwarp();
+            }
+        }
         if (has_matches && warp == 0) {
             for (uint32_t base = 0; base <= mflimit; base += 32) {
                 const uint32_t q = base + lane;
@@ -99,11 +158,23 @@ __device__ __forceinline__ void hc_body(const Params &p) {
                 const uint32_t h = valid ? (load32s(in_s, q) * 2654435761u) >> (32 - kHcHashBits) : 0x80000000u | lane;
                 const unsigned same = __match_any_sync(kFull, h);
                 const unsigned lower = same & ((1u << lane) - 1u);
-                const uint32_t prev = lower ? base + bfind(lower) + 1u : (valid ? lds16(head_s + h * 2u) : 0u);  // position + 1
+                uint32_t dist;
+                if constexpr (kLinked) {  // a head this block has not written is a window position's index (or 0)
+                    const uint32_t hv = valid ? lds16(head_s + h * 2u) : 0u;
+                    const bool mine = valid && ((lds32(bit_s + (h >> 5) * 4u) >> (h & 31u)) & 1u);
+                    dist = lower ? lane - bfind(lower) : !hv ? 0u : mine ? q + 1u - hv : q + kBlock - hv;
+                    if (dist > kHcWindow) dist = 0u;
+                } else {
+                    const uint32_t prev = lower ? base + bfind(lower) + 1u : (valid ? lds16(head_s + h * 2u) : 0u);  // position + 1
+                    dist = prev ? q + 1u - prev : 0u;
+                }
                 __syncwarp();  // every read of head before any update
                 if (valid) {
-                    if ((same >> lane) == 1u) sts16(head_s + h * 2u, q + 1u);  // the highest lane of this hash
-                    sts16(chain_s + q * 2u, prev ? q + 1u - prev : 0u);
+                    if ((same >> lane) == 1u) {  // the highest lane of this hash
+                        sts16(head_s + h * 2u, q + 1u);
+                        if constexpr (kLinked) atomicOr(reinterpret_cast<uint32_t *>(smem + kHcBitOff) + (h >> 5), 1u << (h & 31u));
+                    }
+                    sts16(chain_s + q * 2u, dist);
                 }
                 __syncwarp();
             }
@@ -119,11 +190,16 @@ __device__ __forceinline__ void hc_body(const Params &p) {
                 uint32_t best = 0, boff = 0, c = q, dist = lds16(chain_s + q * 2u);
                 for (uint32_t k = 0; k < kHcDepth && dist; k++) {
                     c -= dist;
+                    if constexpr (kLinked) {
+                        if (q - c > kHcWindow) break;  // (c < 0: a window position)
+                    }
                     // a longer match than `best` must agree at byte `best` (best < cap here): others are skipped unmeasured
-                    if (lds8(in_s + c + best) == lds8(in_s + q + best)) {
+                    const uint32_t cb = kLinked ? load8x(in_s, d.src, (int32_t)(c + best)) : lds8(in_s + c + best);
+                    if (cb == lds8(in_s + q + best)) {
                         uint32_t len = 0;
                         for (;;) {
-                            const uint32_t x = load32s(in_s, q + len) ^ load32s(in_s, c + len);
+                            const uint32_t x = load32s(in_s, q + len) ^
+                                               (kLinked ? load32x(in_s, d.src, (int32_t)(c + len)) : load32s(in_s, c + len));
                             if (x) {
                                 len += (uint32_t)(__ffs(x) - 1) >> 3;
                                 break;
@@ -138,7 +214,8 @@ __device__ __forceinline__ void hc_body(const Params &p) {
                             if (best == cap) break;
                         }
                     }
-                    dist = lds16(chain_s + c * 2u);
+                    if constexpr (kLinked) dist = (int32_t)c >= 0 ? lds16(chain_s + c * 2u) : (uint32_t)__ldcg(g_hist + (c + kBlock));
+                    else dist = lds16(chain_s + c * 2u);
                 }
                 g_len[q] = (uint8_t)(best >= kMinMatch ? best : 0u);
                 g_off[q] = (uint16_t)boff;
@@ -169,7 +246,15 @@ __device__ __forceinline__ void hc_body(const Params &p) {
                         }
                         const uint32_t f = (uint32_t)__ffs(take) - 1u, pos = cur + f;
                         uint32_t ml = __shfl_sync(kFull, len, f);
-                        if (ml == kHcNice) ml = extend_coop_s(in_s, pos, pos - __ldcg(g_off + pos), ml, matchlimit - pos, lane);
+                        if (ml == kHcNice) {
+                            const uint32_t cand = pos - __ldcg(g_off + pos);
+                            if constexpr (kLinked) {
+                                const uint8_t *src = d.src;
+                                ml = extend_coop([in_s, src](uint32_t x) { return load32x(in_s, src, (int32_t)x); }, pos, cand, ml, matchlimit - pos, lane);
+                            } else {
+                                ml = extend_coop_s(in_s, pos, cand, ml, matchlimit - pos, lane);
+                            }
+                        }
                         if (lane == nseq) {
                             q0 = (pos - anchor) | (ml << 16);
                             q1 = anchor | (pos << 16);  // (the offset is fetched for 32 sequences at once when they are emitted)
@@ -209,5 +294,10 @@ __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) {
 // SKY_F_BLOCK_CHECKSUM: the same kernel with block checksums.
 template <uint32_t kHcDepth>
 __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_bc_kernel(const Params p) { hc_body<kHcDepth, true>(p); }
+// SKY_F_LINKED: both with linked blocks (kHcLinkedSmemBytes of shared memory, kHcLinkedScratchBytes of scratch per CTA).
+template <uint32_t kHcDepth>
+__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_linked_kernel(const Params p) { hc_body<kHcDepth, false, true>(p); }
+template <uint32_t kHcDepth>
+__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_linked_bc_kernel(const Params p) { hc_body<kHcDepth, true, true>(p); }
 
 }  // namespace sky

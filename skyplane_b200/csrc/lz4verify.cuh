@@ -18,7 +18,11 @@
 // on its own.  The walk also enforces what liblz4 enforces and the GPU receiver does not (DESIGN §9): off >= 1,
 // q - off >= the block start, no overrun of the block or of the block's bytes, a decoded length of exactly
 // min(64 KiB, n - block start), the last 5 bytes literals and the last match starting >= 12 bytes before the block end.
-// Status 0 therefore means liblz4 decodes the frame to the chunk.  A failure is reported in the receiver's codes, plus
+// Status 0 therefore means liblz4 decodes the frame to the chunk.
+// Linked frames (SKY_F_LINKED, the sky_verify_linked_* kernels): a match may reach back across its block's start, up to
+// the chunk's first byte (off <= block start + q; the 16-bit field caps it at 65535).  The induction still holds per block,
+// since a chunk passes only when every block passes and the earliest failing block's code wins, so the blocks are checked
+// in parallel; the end-of-block rules stay per block.  A failure is reported in the receiver's codes, plus
 // kVerifyMismatch: well formed, but other bytes; within a chunk the earliest failing block's code wins (block_fail, the
 // receiver's per-block status protocol in lz4dec.cuh).
 #pragma once
@@ -51,13 +55,15 @@ struct VerifyParams {
 };
 
 // One thread per chunk: the frame-level checks.  -> kDecOk, kDecChecksum (content checksum: the blocks are still checked,
-// and a block failure takes precedence) or a frame-level code (the blocks are not checked).
+// and a block failure takes precedence) or a frame-level code (the blocks are not checked).  kLinked: the batch's flags
+// may hold SKY_F_LINKED.
+template <bool kLinked>
 __device__ __forceinline__ int32_t verify_frame(const VerifyParams &p, uint32_t c) {
     const ChunkDesc cd = p.chunks[c];
     DecChunk d{cd.dst, nullptr, p.frame_len[c], cd.len, p.blk_base[c], cd.nblk, 0, 0, 0};
     const uint8_t *f = cd.dst;
     uint8_t want[kFrameHeaderBytes];  // the header the stage writes for this chunk
-    write_frame_header(want, cd.len, p.flags);
+    write_frame_header<kLinked>(want, cd.len, p.flags);
     if (d.frame_len >= 11 && (f[4] != want[4] || f[5] != want[5])) return kDecBadHeader;
     int32_t st = kDecOk;
     frame_index(d, p.blocks + d.blk_base, &st);
@@ -97,8 +103,11 @@ __device__ __forceinline__ bool warp_equal(const uint8_t *a, const uint8_t *s, u
 
 // Whole warp, warp-uniform arguments: compare-decode of the compressed block blk[0, slen) against its source block
 // src[0, want) (16-byte aligned).  Every lane walks the same tokens; the lanes compare 32 bytes per round.  A structural
-// failure returns at once; a byte mismatch is only reported once the whole block is known to be well formed.
-__device__ __forceinline__ int32_t compare_decode(const uint8_t *blk, uint32_t slen, const uint8_t *src, uint32_t want, unsigned lane) {
+// failure returns at once; a byte mismatch is only reported once the whole block is known to be well formed.  kLinked:
+// the block starts `pos` bytes into its chunk, whose bytes before src a match may reach.
+template <bool kLinked>
+__device__ __forceinline__ int32_t compare_decode(const uint8_t *blk, uint32_t slen, const uint8_t *src, uint32_t want, uint64_t pos,
+                                                  unsigned lane) {
     bool ok = true;
     uint32_t ip = 0, q = 0;  // q: output position inside the block
     if (slen == 0) return kDecCorrupt;
@@ -115,7 +124,7 @@ __device__ __forceinline__ int32_t compare_decode(const uint8_t *blk, uint32_t s
         if (slen - ip < 2) return kDecCorrupt;
         const uint32_t off = blk[ip] | (blk[ip + 1] << 8);
         ip += 2;
-        if (off == 0 || off > q) return kDecCorrupt;  // q - off before the block start
+        if (off == 0 || (kLinked ? off > pos + q : off > q)) return kDecCorrupt;  // q - off before the block (chunk) start
         uint32_t ml = token & 15;
         if (ml == 15 && !read_ext(blk, slen, ip, ml)) return kDecCorrupt;
         ml += kMinMatch;
@@ -129,6 +138,7 @@ __device__ __forceinline__ int32_t compare_decode(const uint8_t *blk, uint32_t s
 }
 
 // Whole warp: block j of chunk cd as frame_index found it.  -> kDecOk or the block's code.
+template <bool kLinked>
 __device__ __forceinline__ int32_t verify_block(const ChunkDesc &cd, const DecBlock &b, uint32_t j, bool bc, unsigned lane) {
     const uint8_t *blk = cd.dst + b.off;
     const uint32_t sz = b.word & 0x7FFFFFFFu;
@@ -139,24 +149,26 @@ __device__ __forceinline__ int32_t verify_block(const ChunkDesc &cd, const DecBl
         if (sz != want) return kDecLayout;
         return warp_equal(blk, cd.src + pos, sz, lane) ? kDecOk : kVerifyMismatch;
     }
-    return compare_decode(blk, sz, cd.src + pos, want, lane);
+    return compare_decode<kLinked>(blk, sz, cd.src + pos, want, pos, lane);
 }
 
-__global__ void sky_verify_index_kernel(const VerifyParams p) {
+template <bool kLinked>
+__device__ __forceinline__ void verify_index(const VerifyParams &p) {
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c < p.n_chunks) p.status[c] = verify_frame(p, c);
+    if (c < p.n_chunks) p.status[c] = verify_frame<kLinked>(p, c);
 }
 
 // Persistent, one warp per block (work item w = row * n + chunk).  A block is skipped once the frame or an earlier block
 // of its chunk has failed.
-__global__ void __launch_bounds__(kVerifyThreads, 2) sky_verify_kernel(const VerifyParams p) {
+template <bool kLinked>
+__device__ __forceinline__ void verify_blocks(const VerifyParams &p) {
     const unsigned lane = threadIdx.x & 31;
     const bool bc = (p.flags & SKY_F_BLOCK_CHECKSUM) != 0;
     for (uint32_t c, j; claim_row_major(p.counter, p.n_chunks, p.rows, lane, c, j);) {
         const ChunkDesc cd = p.chunks[c];
         if (j >= cd.nblk) continue;
         if (!block_may_run(*reinterpret_cast<volatile int32_t *>(p.status + c), j)) continue;
-        const int32_t r = verify_block(cd, p.blocks[p.blk_base[c] + j], j, bc, lane);
+        const int32_t r = verify_block<kLinked>(cd, p.blocks[p.blk_base[c] + j], j, bc, lane);
         if (r != kDecOk && lane == 0) atomicMin(p.status + c, block_fail(j, r));
     }
 }
@@ -165,7 +177,8 @@ __global__ void __launch_bounds__(kVerifyThreads, 2) sky_verify_kernel(const Ver
 // the stage's header (write_frame_header), every block stored raw from the chunk (with its block checksum under
 // SKY_F_BLOCK_CHECKSUM), the EndMark and the content checksum (finish_frame) -- frame_need(n, flags) bytes, which the
 // frame's capacity holds.
-__global__ void __launch_bounds__(kRepairWarps * 32) sky_verify_settle_kernel(const VerifyParams p) {
+template <bool kLinked>
+__device__ __forceinline__ void verify_settle(const VerifyParams &p) {
     __shared__ int32_t code;
     const uint32_t c = blockIdx.x;
     const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -187,12 +200,20 @@ __global__ void __launch_bounds__(kRepairWarps * 32) sky_verify_settle_kernel(co
         if (bc && warp == j % kRepairWarps) block_checksum(cd.src + pos, L, w + 4 + L, lane);  // (the same bytes, from the chunk)
     }
     if (threadIdx.x == 0) {
-        write_frame_header(cd.dst, cd.len, p.flags);
+        write_frame_header<kLinked>(cd.dst, cd.len, p.flags);
         uint8_t *e = cd.dst + hdr + (uint64_t)cd.nblk * (4 + bc) + cd.len;
         st_u32le(e, 0);  // EndMark
         p.frame_len[c] = (uint64_t)(e - cd.dst) + 4;
         if (p.flags & SKY_F_CHECKSUM) finish_frame(cd.dst, p.frame_len + c, p.xxh[c]);
     }
 }
+
+__global__ void sky_verify_index_kernel(const VerifyParams p) { verify_index<false>(p); }
+__global__ void __launch_bounds__(kVerifyThreads, 2) sky_verify_kernel(const VerifyParams p) { verify_blocks<false>(p); }
+__global__ void __launch_bounds__(kRepairWarps * 32) sky_verify_settle_kernel(const VerifyParams p) { verify_settle<false>(p); }
+// SKY_F_LINKED: the same three for linked frames
+__global__ void sky_verify_linked_index_kernel(const VerifyParams p) { verify_index<true>(p); }
+__global__ void __launch_bounds__(kVerifyThreads, 2) sky_verify_linked_kernel(const VerifyParams p) { verify_blocks<true>(p); }
+__global__ void __launch_bounds__(kRepairWarps * 32) sky_verify_linked_settle_kernel(const VerifyParams p) { verify_settle<true>(p); }
 
 }  // namespace sky

@@ -605,7 +605,7 @@ struct BatchMeta {  // one batch's descriptors and results (the receiver uses th
     DevMem<uint8_t> scratch;  // compress scratch: kScratchBytes per CTA of the grid (kernels of different slots overlap)
 };
 struct HcArrays {  // SKY_F_HC: the HC kernel's scratch, and the stream the digests run on beside it (fork / join events)
-    DevMem<uint8_t> scratch;  // kHcScratchBytes per CTA (one CTA per SM)
+    DevMem<uint8_t> scratch;  // kHcLinkedScratchBytes per CTA (one CTA per SM; kHcScratchBytes of it without SKY_F_LINKED)
     Stream md5_stream;
     Event ev_fork, ev_join;
 };
@@ -620,6 +620,17 @@ static const HcKernel kHcBcKernels[] = {sky_hc_bc_kernel<hc_depth(3)>, sky_hc_bc
                                         sky_hc_bc_kernel<hc_depth(6)>, sky_hc_bc_kernel<hc_depth(7)>, sky_hc_bc_kernel<hc_depth(8)>,
                                         sky_hc_bc_kernel<hc_depth(9)>};
 static_assert(sizeof(kHcBcKernels) == sizeof(kHcKernels), "one HC kernel with block checksums per level");
+// ... and both with linked blocks (SKY_F_LINKED)
+static const HcKernel kHcLinkedKernels[] = {sky_hc_linked_kernel<hc_depth(3)>, sky_hc_linked_kernel<hc_depth(4)>,
+                                            sky_hc_linked_kernel<hc_depth(5)>, sky_hc_linked_kernel<hc_depth(6)>,
+                                            sky_hc_linked_kernel<hc_depth(7)>, sky_hc_linked_kernel<hc_depth(8)>,
+                                            sky_hc_linked_kernel<hc_depth(9)>};
+static const HcKernel kHcLinkedBcKernels[] = {sky_hc_linked_bc_kernel<hc_depth(3)>, sky_hc_linked_bc_kernel<hc_depth(4)>,
+                                              sky_hc_linked_bc_kernel<hc_depth(5)>, sky_hc_linked_bc_kernel<hc_depth(6)>,
+                                              sky_hc_linked_bc_kernel<hc_depth(7)>, sky_hc_linked_bc_kernel<hc_depth(8)>,
+                                              sky_hc_linked_bc_kernel<hc_depth(9)>};
+static_assert(sizeof(kHcLinkedKernels) == sizeof(kHcKernels) && sizeof(kHcLinkedBcKernels) == sizeof(kHcKernels),
+              "one linked HC kernel, with and without block checksums, per level");
 constexpr uint32_t kHcLevelShift = 8, kHcLevelMask = 0xfu << kHcLevelShift;  // SKY_F_HC_LEVEL's field in `flags`
 static_assert(SKY_F_HC_LEVEL(1) == (SKY_F_HC | (1u << kHcLevelShift)), "the level field of include/skychunk.h");
 // The level a batch's flags select: the level field, or kHcDefaultLevel when it is 0.
@@ -757,7 +768,7 @@ static int alloc_dec(sky_ctx *ctx, DecodeArrays &d) {
 static int alloc_hc(sky_ctx *ctx, HcArrays &h) {
     if (h.scratch) return SKY_OK;
     HcArrays a;
-    CK(ctx, cudaMalloc(a.scratch.put(), (size_t)ctx->sm_count * kHcScratchBytes));
+    CK(ctx, cudaMalloc(a.scratch.put(), (size_t)ctx->sm_count * kHcLinkedScratchBytes));
     CK(ctx, cudaStreamCreateWithFlags(a.md5_stream.put(), cudaStreamNonBlocking));
     CK(ctx, cudaEventCreateWithFlags(a.ev_fork.put(), cudaEventDisableTiming));
     CK(ctx, cudaEventCreateWithFlags(a.ev_join.put(), cudaEventDisableTiming));
@@ -914,6 +925,10 @@ int sky_ctx_create(int device, uint64_t max_batch_bytes, uint32_t max_chunks, ui
         if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
     for (const HcKernel k : kHcBcKernels)
         if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
+    for (const HcKernel k : kHcLinkedKernels)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcLinkedSmemBytes);
+    for (const HcKernel k : kHcLinkedBcKernels)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcLinkedSmemBytes);
     if (e != cudaSuccess) {
         g_err = ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (this build carries sm_90a code only)";
         return SKY_E_CUDA;
@@ -1033,9 +1048,11 @@ static uint32_t fill_md5_order(uint32_t *order, uint32_t n, const uint64_t *len)
 
 // SKY_F_HC selects how frames are made, SKY_F_CHECKSUM / SKY_F_BLOCK_CHECKSUM add to the frame and SKY_F_VERIFY checks
 // it, so each needs SKY_F_LZ4, or no stage bit at all (= LZ4 + MD5).  A level field needs SKY_F_HC and a level in kHcMinLevel .. kHcMaxLevel.
+// SKY_F_LINKED needs SKY_F_HC: only the high-ratio compressor links blocks.
 static bool frame_flags_valid(uint32_t flags) {
     if ((flags & kHcLevelMask) && (!(flags & SKY_F_HC) || hc_level(flags) < kHcMinLevel || hc_level(flags) > kHcMaxLevel))
         return false;
+    if ((flags & SKY_F_LINKED) && !(flags & SKY_F_HC)) return false;
     return !(flags & (SKY_F_HC | SKY_F_CHECKSUM | SKY_F_BLOCK_CHECKSUM | SKY_F_VERIFY)) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5;
 }
 // Bytes a chunk's frame may take: SKY_F_CHECKSUM adds the 4-byte content checksum behind the EndMark,
@@ -1075,11 +1092,12 @@ static int launch_verify(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, uin
     p.rows = rows;
     p.flags = flags;
     p.repair = repair ? 1u : 0u;
-    sky_verify_index_kernel<<<(n + 127) / 128, 128, 0, st>>>(p);
+    const bool linked = (flags & SKY_F_LINKED) != 0;
+    (linked ? sky_verify_linked_index_kernel : sky_verify_index_kernel)<<<(n + 127) / 128, 128, 0, st>>>(p);
     CK(ctx, cudaGetLastError());
-    sky_verify_kernel<<<ctx->sm_count * 2, kVerifyThreads, 0, st>>>(p);
+    (linked ? sky_verify_linked_kernel : sky_verify_kernel)<<<ctx->sm_count * 2, kVerifyThreads, 0, st>>>(p);
     CK(ctx, cudaGetLastError());
-    sky_verify_settle_kernel<<<n, kRepairWarps * 32, 0, st>>>(p);
+    (linked ? sky_verify_linked_settle_kernel : sky_verify_settle_kernel)<<<n, kRepairWarps * 32, 0, st>>>(p);
     CK(ctx, cudaGetLastError());
     ctx->launches += 3;
     return SKY_OK;
@@ -1154,7 +1172,11 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
             ctx->launches++;
         }
         p.scratch = h.scratch;
-        (bc ? kHcBcKernels : kHcKernels)[hc_level(flags) - kHcMinLevel]<<<ctx->sm_count, kHcThreads, kHcSmemBytes, st>>>(p);
+        const int lv = hc_level(flags) - kHcMinLevel;
+        if (flags & SKY_F_LINKED)
+            (bc ? kHcLinkedBcKernels : kHcLinkedKernels)[lv]<<<ctx->sm_count, kHcThreads, kHcLinkedSmemBytes, st>>>(p);
+        else
+            (bc ? kHcBcKernels : kHcKernels)[lv]<<<ctx->sm_count, kHcThreads, kHcSmemBytes, st>>>(p);
         CK(ctx, cudaGetLastError());
         if (md5) CK(ctx, cudaStreamWaitEvent(st, h.ev_join, 0));
     } else {

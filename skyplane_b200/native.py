@@ -16,6 +16,7 @@ SKY_OK = 0
 SKY_E_INVALID, SKY_E_NOGPU, SKY_E_CUDA, SKY_E_CAPACITY, SKY_E_BUSY, SKY_E_TICKET, SKY_E_NOMEM, SKY_E_NOKEY = -1, -2, -3, -4, -5, -6, -7, -8
 F_LZ4, F_MD5, F_E2EE, F_HC, F_CHECKSUM, F_BLOCK_CHECKSUM = 1, 2, 16, 32, 64, 128
 F_VERIFY = 1 << 12  # every frame is checked against its chunk on the GPU; one that fails is sent as its stored-block frame
+F_LINKED = 1 << 13  # with F_HC only: linked blocks (python-lz4's block_linked), matches may reach into the previous 64 KiB
 CHECKSUM_BYTES = 4  # F_CHECKSUM: the content checksum (u32le XXH32) behind the EndMark; F_BLOCK_CHECKSUM: as many per block
 BLOCK_BYTES = 65536
 # SKY_F_HC_LEVEL(l): the high-ratio level l (3..9: 2**(l - 1) chain candidates per position) in bits 8..11 of the flags;
@@ -196,12 +197,12 @@ def frame_need(n: int, checksum: bool = False, block_checksum: bool = False) -> 
 
 
 _DECODE_ONLY_SUBMIT = ((F_HC, "F_HC"), (HC_LEVEL_MASK, "a high-ratio level"), (F_CHECKSUM, "F_CHECKSUM"),
-                       (F_BLOCK_CHECKSUM, "F_BLOCK_CHECKSUM"), (F_VERIFY, "F_VERIFY"))
+                       (F_BLOCK_CHECKSUM, "F_BLOCK_CHECKSUM"), (F_VERIFY, "F_VERIFY"), (F_LINKED, "F_LINKED"))
 
 
 def check_decode_flags(flags: int) -> int:
-    """sky_decode takes the stage bits (F_LZ4, F_MD5) and F_E2EE only: a frame says itself which checksums it carries, and
-    the compressor that made it does not matter to a decoder.  -> flags, or a ValueError naming the bit it does not take."""
+    """sky_decode takes the stage bits (F_LZ4, F_MD5) and F_E2EE only: a frame says itself which checksums it carries and
+    whether its blocks are linked, and the compressor that made it does not matter to a decoder.  -> flags, or a ValueError naming the bit it does not take."""
     for bit, name in _DECODE_ONLY_SUBMIT:
         if flags & bit:
             raise ValueError(f"decode does not take {name}: it is a sender option (flags {flags:#x})")

@@ -141,6 +141,7 @@ class GatewayCompressHash(GatewayOperator):
         compression_level: Optional[int] = None,
         block_checksum: bool = False,
         verify_frames: bool = False,
+        block_linked: bool = False,
     ):
         """use_compression / e2ee_key_bytes: GatewaySender's arguments of the same name (gateway_operator.py:154-168):
         ``use_compression=False`` digests the chunk and lets it pass through uncompressed (``is_compressed=False``);
@@ -158,6 +159,9 @@ class GatewayCompressHash(GatewayOperator):
         verify_frames: the GPU checks every frame against its chunk before it leaves (``ChunkStage.launch(verify=True)``); a
         frame that would not restore the chunk is sent as the chunk's stored-block frame instead, a warning names the chunk
         and the failed check, and the chunk's ``complete`` record carries ``frame_verify_status``.  Needs ``use_compression``.
+        block_linked: python-lz4's argument of the same name, for the high-ratio parse (``ChunkStage.launch(linked=True)``): a
+        match may reach up to 65535 bytes back into the chunk's previous block, which saves bytes on text.  The default stays
+        independent blocks.  Needs ``high_ratio`` or a ``compression_level`` of 3..9.
         sink: ``callable(worker_id) -> socket``, called once in each worker.  With a sink the worker sends every payload
         straight from the pinned staging slot (``wire.send_results``: WireProtocolHeader + payload, no intermediate bytes
         object, no frame file) -- the tail of ``GatewaySender.process`` (gateway_operator.py:367-402)."""
@@ -177,7 +181,10 @@ class GatewayCompressHash(GatewayOperator):
         self.verify_frames = bool(verify_frames)
         from skyplane_b200 import native
 
-        native.hc_flags(compression_level, self.high_ratio, self.use_compression)  # (ValueError on a bad level, here and not in a worker)
+        hc_bits = native.hc_flags(compression_level, self.high_ratio, self.use_compression)  # (ValueError on a bad level, here and not in a worker)
+        if block_linked and not hc_bits:
+            raise ValueError("block_linked is a mode of the high-ratio compressor: it needs high_ratio or a compression_level of 3..9")
+        self.block_linked = bool(block_linked)
         self.compression_level = compression_level
         self.e2ee_key_bytes = e2ee_key_bytes
         self.sink = sink
@@ -330,6 +337,8 @@ class GatewayCompressHash(GatewayOperator):
             opts["block_checksum"] = True
         if self.verify_frames:
             opts["verify"] = True
+        if self.block_linked:
+            opts["linked"] = True
         stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None, **opts)
         return True
 

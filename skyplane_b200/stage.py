@@ -44,6 +44,12 @@ def _out_room(n: int) -> int:
     return native.round16(native.frame_need(n, checksum=True, block_checksum=True) + native.BOX_OVERHEAD)
 
 
+def _check_linked(linked: bool, hc_bits: int):
+    """linked=True (F_LINKED) needs the high-ratio mode: the fast compressor has no linked-block mode (DESIGN §4.2)."""
+    if linked and not hc_bits:
+        raise ValueError("linked=True is a mode of the high-ratio compressor: it needs hc=True or a level 3..9")
+
+
 class _Slot:
     def __init__(self, in_bytes: int, out_bytes: int):
         self.inp = native.PinnedBuffer(in_bytes)
@@ -164,7 +170,8 @@ class ChunkStage:
         self._has_key = key is not None
 
     def launch(self, slot: _Slot, compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None, hc: bool = False,
-               checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False, verify: bool = False) -> _Slot:
+               checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False, verify: bool = False,
+               linked: bool = False) -> _Slot:
         """compress=False is the reference's `compress: false` (digest only, the chunk passes through);
         encrypt=True seals every payload with the stage's key (nonces: 24 bytes per chunk, default os.urandom);
         hc=True makes the frames with the high-ratio parse (F_HC): same frame format, fewer bytes, more GPU time;
@@ -175,7 +182,10 @@ class ChunkStage:
         candidates per position: more ratio for more GPU time), hc=True alone means level 5, 0..2 is the fast path;
         verify=True checks every frame against its chunk on the GPU before it is sealed or copied out (F_VERIFY): a frame
         that would not restore the chunk is replaced by the chunk's stored-block frame and its StageResult.verify_status
-        says why."""
+        says why;
+        linked=True is python-lz4's block_linked for the high-ratio parse (F_LINKED): a match may reach up to 65535 bytes
+        back into the chunk's previous block, which saves bytes on text; the receiver decodes such a frame's blocks in
+        order.  It needs the high-ratio mode (hc=True or a level 3..9)."""
         if not slot.lens:
             raise ValueError("empty batch")
         if hc and not compress:
@@ -187,6 +197,7 @@ class ChunkStage:
         if verify and not compress:
             raise ValueError("verify=True checks the LZ4 frames: it needs compress=True")
         hc_bits = native.hc_flags(level, hc, compress)
+        _check_linked(linked, hc_bits)
         if hc_bits and not native.kernel_config()["hc_depth"]:
             raise native.SkyChunkError(native.SKY_E_INVALID, f"{native.LIB_PATH.name} was built without the high-ratio kernel (F_HC)")
         if hc_bits & native.HC_LEVEL_MASK and native.kernel_config()["hc_max_level"] < level:
@@ -195,7 +206,7 @@ class ChunkStage:
         src = [base_in + o for o in slot.in_off]
         flags = (native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0) | hc_bits
                  | (native.F_CHECKSUM if checksum else 0) | (native.F_BLOCK_CHECKSUM if block_checksum else 0)
-                 | (native.F_VERIFY if verify else 0))
+                 | (native.F_VERIFY if verify else 0) | (native.F_LINKED if linked else 0))
         if encrypt and nonces is None:
             nonces = os.urandom(24 * len(slot.lens))  # what nacl.utils.random(24) draws per message
         if compress or encrypt:
@@ -227,10 +238,10 @@ class ChunkStage:
     # ------------------------------------------------------------------ sync convenience
     def process(self, chunks: Sequence[BytesLike], compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None,
                 hc: bool = False, checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False,
-                verify: bool = False) -> List[StageResult]:
+                verify: bool = False, linked: bool = False) -> List[StageResult]:
         """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes (hc, checksum,
-        level, block_checksum, verify: see launch)."""
-        native.hc_flags(level, hc, compress)  # (bad arguments fail before the first batch)
+        level, block_checksum, verify, linked: see launch)."""
+        _check_linked(linked, native.hc_flags(level, hc, compress))  # (bad arguments fail before the first batch)
         if block_checksum and not compress:
             raise ValueError("block_checksum=True is carried by the LZ4 frame: it needs compress=True")
         if verify and not compress:
@@ -247,7 +258,7 @@ class ChunkStage:
                 self.release(slot)
                 raise native.SkyChunkError(native.SKY_E_CAPACITY, f"chunk of {memoryview(chunks[i]).nbytes} bytes exceeds max_batch_bytes")
             self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum, level, block_checksum,
-                        verify)
+                        verify, linked)
             for r in self.collect(slot):
                 out.append(StageResult(frame=memoryview(bytes(r.frame)), md5=r.md5, raw_len=r.raw_len, comp_len=r.comp_len,
                                        is_compressed=r.is_compressed, is_encrypted=r.is_encrypted, verify_status=r.verify_status))

@@ -1,5 +1,6 @@
 """Python face of tools/lz4hc_model.c, the sequential CPU twin of the high-ratio (SKY_F_HC) block compressor (development /
-test tool, not product code).  frame(data) is the LZ4 frame the GPU stage must emit byte for byte with SKY_F_HC."""
+test tool, not product code).  frame(data) is the LZ4 frame the GPU stage must emit byte for byte with SKY_F_HC, and
+frame(data, linked=True) the one it emits with SKY_F_HC | SKY_F_LINKED."""
 from __future__ import annotations
 
 import ctypes
@@ -37,23 +38,33 @@ def lib():
         _lib = ctypes.CDLL(str(_SO))
         _lib.hc_compress_block.argtypes = [ctypes.c_char_p, ctypes.c_uint32, ctypes.c_char_p, ctypes.POINTER(Opts)]
         _lib.hc_compress_block.restype = ctypes.c_uint32
+        _lib.hc_compress_block_linked.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_char_p, ctypes.POINTER(Opts)]
+        _lib.hc_compress_block_linked.restype = ctypes.c_uint32
     return _lib
 
 
-def blocks(data: bytes, o: Opts):
-    """-> list of (compressed size or 0 when stored raw, block bytes as they appear in the frame)."""
+WINDOW = 65536  # linked: source bytes before a block (after the chunk's first) that its matches may reach
+
+
+def blocks(data: bytes, o: Opts, linked: bool = False):
+    """-> list of (compressed size or 0 when stored raw, block bytes as they appear in the frame).  linked: blocks after
+    the first see the previous 64 KiB of the chunk (hc_compress_block_linked)."""
     L = lib()
     buf = ctypes.create_string_buffer(65536 + 4096)
+    src = ctypes.create_string_buffer(bytes(data), len(data)) if linked else None
     out = []
     for pos in range(0, len(data), 65536):
         blk = data[pos:pos + 65536]
-        c = L.hc_compress_block(blk, len(blk), buf, ctypes.byref(o))
+        if linked:
+            c = L.hc_compress_block_linked(ctypes.addressof(src) + pos, len(blk), min(pos, WINDOW), buf, ctypes.byref(o))
+        else:
+            c = L.hc_compress_block(blk, len(blk), buf, ctypes.byref(o))
         out.append((c, buf.raw[:c] if c else blk))
     return out
 
 
-def frame(data: bytes, o: Opts | None = None, block_checksum: bool = False) -> bytes:
-    return tile_model.assemble(len(data), blocks(data, o or kernel_opts()), block_checksum)
+def frame(data: bytes, o: Opts | None = None, block_checksum: bool = False, linked: bool = False) -> bytes:
+    return tile_model.assemble(len(data), blocks(data, o or kernel_opts(), linked), block_checksum, linked)
 
 
 def liblz4_frame(data: bytes, level: int, linked: bool = False, content_checksum: bool = False, block_checksum: bool = False) -> bytes:

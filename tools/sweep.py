@@ -5,7 +5,9 @@ Flag sets: lz4, md5, both (the fused kernel), hc (SKY_F_HC: high-ratio frames + 
 checksum / hc-checksum (SKY_F_CHECKSUM: frames with LZ4's content checksum, fast or high-ratio), hc3 .. hc9 and
 hc3-checksum .. hc9-checksum (SKY_F_HC_LEVEL(3..9): the high-ratio mode at that level; hc5 makes hc's frames);
 block-checksum, block-checksum-checksum, hc-block-checksum, hc-block-checksum-checksum and hc3-block-checksum ..
-hc9-block-checksum (SKY_F_BLOCK_CHECKSUM: the same frames with LZ4's block checksums, alone or with the content checksum).
+hc9-block-checksum (SKY_F_BLOCK_CHECKSUM: the same frames with LZ4's block checksums, alone or with the content checksum);
+hc-linked, hc3-linked .. hc9-linked and their -checksum / -block-checksum forms (SKY_F_LINKED: the high-ratio frames with
+linked blocks).
 --decode-from liblz4[-linked][-checksums] times the receiver on liblz4's level-0 frames made on the host from the same
 input: independent or linked blocks, without checksums or with block and content checksums.
 --ref-ratio adds the reference's ratio (liblz4 level 0, linked blocks) on the distinct chunks; --liblz4-level9 times liblz4
@@ -190,6 +192,9 @@ def main():
         FL[f"hc{lv}"] = native.hc_level_flag(lv)
         FL[f"hc{lv}-checksum"] = native.hc_level_flag(lv) | native.F_CHECKSUM
         FL[f"hc{lv}-block-checksum"] = native.hc_level_flag(lv) | native.F_BLOCK_CHECKSUM
+    for k in [k for k in FL if k.startswith("hc") and k != "hc-lz4"]:  # hc5-checksum -> hc5-linked-checksum
+        head, _, tail = k.partition("-")
+        FL[f"{head}-linked" + (f"-{tail}" if tail else "")] = FL[k] | native.F_LINKED
     FL.update({"block-checksum": native.F_BLOCK_CHECKSUM, "block-checksum-checksum": native.F_BLOCK_CHECKSUM | native.F_CHECKSUM,
                "hc-block-checksum": native.F_HC | native.F_BLOCK_CHECKSUM,
                "hc-block-checksum-checksum": native.F_HC | native.F_BLOCK_CHECKSUM | native.F_CHECKSUM})
