@@ -6,8 +6,9 @@
 //   LOP3 (F/G/H/I of the newest b) -> IADD3 (+ (a + M[g]) + K[i]; a + M[g] is an IMAD on the FMA pipe, off the chain)
 //   -> LEA.HI (b + rotl(t, s): ptxas fuses the funnel shift and the add).
 // Each ALU -> ALU hop is 4 cycles, so a step is scheduled at 12 (tools/md5_schedule.py reads it from the SASS).
-// Message words are staged into shared memory with 16-byte cp.async SKY_MD5_SLOTS-1 blocks ahead of the
-// chain (ring of SKY_MD5_SLOTS x 64 B per lane, laid out [slot][piece][lane] so LDS.128 is conflict-free).
+// Message words are staged into shared memory with 16-byte cp.async a ring's depth of blocks ahead of the chain (ring of
+// kSlots x 64 B per lane, laid out [slot][piece][lane] so LDS.128 is conflict-free): SKY_MD5_SLOTS = 8 on the sender,
+// whose copies compete with the compressors' stream, 4 on the receiver.
 #pragma once
 #include <stdint.h>
 #include "xxh32.cuh"
@@ -15,10 +16,52 @@
 #include <utility>
 
 #ifndef SKY_MD5_SLOTS
-#define SKY_MD5_SLOTS 4
+#define SKY_MD5_SLOTS 8
 #endif
 
 namespace sky {
+
+#ifdef SKY_MD5_TRACE
+// Diagnostic build only (tools/build_variants.py md5_trace, read by tools/md5_trace.py): lane 0 of each sender MD5 warp
+// stamps %globaltimer and %clock at its group's start and end and every kTraceEvery blocks, and sums the cycles the warp
+// spends in the ring's cp.async wait.  The default build has none of this.
+constexpr int kTraceGroups = 256, kTraceStamps = 512, kTraceEvery = 1024;
+struct Md5TraceStamp {
+    uint64_t t;     // %globaltimer (ns)
+    uint32_t clk;   // %clock
+    uint32_t wait;  // ring-wait cycles so far
+};
+struct Md5Trace {
+    uint32_t smid, warpid, cta, stamps;
+    uint64_t t0, t1;
+    uint32_t c0, c1, wait, blocks;
+    Md5TraceStamp s[kTraceStamps];  // s[k]: after block (k + 1) * kTraceEvery
+};
+__device__ Md5Trace g_md5_trace[kTraceGroups];
+__device__ __forceinline__ uint64_t trace_globaltimer() {
+    uint64_t t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+__device__ __forceinline__ uint32_t trace_clock() {
+    uint32_t c;
+    asm volatile("mov.u32 %0, %%clock;" : "=r"(c));
+    return c;
+}
+__device__ __forceinline__ uint32_t trace_smid() {
+    uint32_t s;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+    return s;
+}
+__device__ __forceinline__ uint32_t trace_warpid() {
+    uint32_t w;
+    asm volatile("mov.u32 %0, %%warpid;" : "=r"(w));
+    return w;
+}
+#define SKY_MD5_TRACE_PARAM , Md5Trace *trace = nullptr
+#else
+#define SKY_MD5_TRACE_PARAM
+#endif
 
 struct Md5State {
     uint32_t a, b, c, d;
@@ -181,7 +224,7 @@ __device__ __forceinline__ void md5_unroll(F &&f) {
 
 // md5_warp<true> also runs XXH32 (the LZ4 content checksum) over the same words: one 16-byte stripe after each MD5 round,
 // where its four short chains fill issue slots the MD5 chain leaves idle.
-// Digest of one chunk per lane.  `ring` = this warp's 8 KiB shared-memory area (2048 x uint32),
+// Digest of one chunk per lane.  `ring` = this warp's kSlots x 2 KiB shared-memory area,
 // `src` 16-byte aligned (or len == 0), `active` false for lanes without a chunk.
 // Writes 16 digest bytes to `out` for active lanes.  kXxh: also returns XXH32(chunk, seed 0) (0 without kXxh or when
 // the lane is inactive).
@@ -191,17 +234,21 @@ struct Md5NoGate {
     __device__ __forceinline__ void operator()(uint64_t, bool) const {}
 };
 
-template <bool kXxh = false, class Gate = Md5NoGate>
+template <bool kXxh = false, class Gate = Md5NoGate, int kSlots = SKY_MD5_SLOTS>
 __device__ __forceinline__ uint32_t md5_warp(uint32_t *ring, const uint8_t *src, uint64_t len, bool active, uint8_t *out,
-                                             unsigned lane, Gate gate = Gate()) {
-    constexpr int kSlots = SKY_MD5_SLOTS;  // ring depth (blocks, power of two); prefetch distance = kSlots - 1
-    static_assert(kSlots >= 2 && (kSlots & (kSlots - 1)) == 0 && 1024 % kSlots == 0, "SKY_MD5_SLOTS: a power of two, 2..1024");
+                                             unsigned lane, Gate gate = Gate() SKY_MD5_TRACE_PARAM) {
+    // kSlots: ring depth in blocks and the prefetch distance -- block i + kSlots is staged into block i's slot while block
+    // i is hashed (its words are in registers by then).  The loop body is kUnroll blocks whatever the depth: a deeper
+    // ring only moves where the copies land, not the chain's instruction stream.
+    constexpr int kUnroll = 4;
+    static_assert((kSlots & (kSlots - 1)) == 0 && kSlots % kUnroll == 0 && 1024 % kSlots == 0,
+                  "the MD5 ring: a power of two, a multiple of 4 and at most 1024 blocks");
     constexpr bool kGated = !std::is_same<Gate, Md5NoGate>::value;
     // Block counts are 32-bit: the host rejects chunks over 128 GiB (kMaxChunkBlocks in skychunk.cu), so nfull <= 2^31
-    // and the trip count rounded up to kSlots cannot wrap.
+    // and the trip count rounded up to kUnroll cannot wrap.
     const uint32_t nfull = active ? (uint32_t)(len >> 6) : 0;
     const uint32_t wmax = __reduce_max_sync(0xffffffffu, nfull);
-    const uint32_t trips = (wmax + (kSlots - 1)) & ~(uint32_t)(kSlots - 1);
+    const uint32_t trips = (wmax + (kUnroll - 1)) & ~(uint32_t)(kUnroll - 1);
     Md5State st;  // runs on through the blocks past this lane's end (the loop has no branch per lane) ...
     md5_init(st);
     Md5State fin = st;  // ... so the state after the lane's last full block is kept here, off the chain
@@ -214,17 +261,28 @@ __device__ __forceinline__ uint32_t md5_warp(uint32_t *ring, const uint8_t *src,
     const uint32_t *lring = ring + lane * 4;
     const uint32_t lring_s = (uint32_t)__cvta_generic_to_shared(lring);
     const uint32_t one = md5_one();
+#ifdef SKY_MD5_TRACE
+    uint32_t wait_cycles = 0;
+    if (trace && lane == 0) {
+        trace->smid = trace_smid();
+        trace->warpid = trace_warpid();
+        trace->cta = blockIdx.x;
+        trace->t0 = trace_globaltimer();
+        trace->c0 = trace_clock();
+    }
+#endif
 
     gate(0, active && len > 0);
-    md5_unroll<kSlots - 1>([&](auto sc) {
+    md5_unroll<kSlots>([&](auto sc) {
         constexpr int s = decltype(sc)::value;
         cp_async_block<s>((uint32_t)s < nfull, lring_s, src + s * 64);
         cp_async_commit();
     });
-    auto load_words = [&](uint32_t (&w)[16], int cs) {
+    // the words of the block in the slot at byte offset `so` of the ring (a multiple of 2 KiB)
+    auto load_words = [&](uint32_t (&w)[16], uint32_t so) {
 #pragma unroll
         for (int q = 0; q < 4; q++) {
-            const uint4 v = *reinterpret_cast<const uint4 *>(lring + (cs * 4 + q) * 128);
+            const uint4 v = *reinterpret_cast<const uint4 *>(lring + so / 4 + q * 128);
             w[4 * q + 0] = v.x;
             w[4 * q + 1] = v.y;
             w[4 * q + 2] = v.z;
@@ -235,16 +293,16 @@ __device__ __forceinline__ uint32_t md5_warp(uint32_t *ring, const uint8_t *src,
     // chain runs.  Every lane hashes every block up to `trips`; a lane past its end hashes stale ring words and keeps
     // only `fin`.
     uint32_t w[2][16];
-    cp_async_wait<kSlots - 2>();  // block 0 has landed
+    cp_async_wait<kSlots - 1>();  // block 0 has landed
     load_words(w[0], 0);
-    const uint8_t *pf_src = src + (kSlots - 1) * 64;  // block i + kSlots - 1, the next one to stage
-    // Blocks i .. i + kSlots - 1 (i a multiple of kSlots) as one branch-free stretch: the staging sits between the
-    // rounds, where ptxas can issue it in the chain's idle cycles.
+    const uint8_t *pf_src = src + kSlots * 64;  // block i + kSlots, the next one to stage
+    // Blocks i .. i + kUnroll - 1 (i a multiple of kUnroll) as one branch-free stretch: the staging sits between the
+    // rounds, where ptxas can issue it in the chain's idle cycles.  Their slots are consecutive from block i's, so each
+    // is the stretch's ring offset (off the chain, once per stretch) plus an immediate.
     auto blocks = [&](uint32_t i) {
-        md5_unroll<kSlots>([&](auto uc) {
+        const uint32_t so = (i & (kSlots - 1)) * 2048, so_next = ((i + kUnroll) & (kSlots - 1)) * 2048;
+        md5_unroll<kUnroll>([&](auto uc) {
             constexpr int u = decltype(uc)::value;
-            constexpr int ps = (u + kSlots - 1) & (kSlots - 1);  // slot of block i+u-1, read during block i+u-2
-            constexpr int ns = (u + 1) & (kSlots - 1);
             uint32_t a = st.a, b = st.b, c = st.c, d = st.d;
             const uint32_t(&wu)[16] = w[u & 1];
             auto stripe = [&](int q) {
@@ -252,14 +310,20 @@ __device__ __forceinline__ uint32_t md5_warp(uint32_t *ring, const uint8_t *src,
             };
             md5_round<0>(a, b, c, d, wu, one);
             stripe(0);
-            cp_async_block<ps>(i + u + (kSlots - 1) < nfull, lring_s, pf_src + u * 64);
+            cp_async_block<u>(i + u + kSlots < nfull, lring_s + so, pf_src + u * 64);  // block i+u+kSlots into block i+u's slot
             md5_round<1>(a, b, c, d, wu, one);
             stripe(1);
             cp_async_commit();
-            cp_async_wait<kSlots - 2>();  // block i+u+1 has landed
+#ifdef SKY_MD5_TRACE
+            const uint32_t wait_from = trace_clock();
+#endif
+            cp_async_wait<kSlots - 1>();  // block i+u+1 has landed
+#ifdef SKY_MD5_TRACE
+            wait_cycles += trace_clock() - wait_from;
+#endif
             md5_round<2>(a, b, c, d, wu, one);
             stripe(2);
-            load_words(w[(u + 1) & 1], ns);
+            load_words(w[(u + 1) & 1], u + 1 < kUnroll ? so + (u + 1) * 2048 : so_next);
             md5_round<3>(a, b, c, d, wu, one);
             stripe(3);
             st.a += a;
@@ -271,21 +335,37 @@ __device__ __forceinline__ uint32_t md5_warp(uint32_t *ring, const uint8_t *src,
                 if constexpr (kXxh) xfin = xs;
             }
         });
-        pf_src += kSlots * 64;
+        pf_src += kUnroll * 64;
     };
     if constexpr (kGated) {
         // Receiver side: a row-granular outer loop keeps the gate (a spin with a scheduling barrier) out of the
-        // chain-bound inner loop; the prefetch runs kSlots-1 blocks ahead, so a row is gated one row early.  A row
-        // (1024 blocks) is a whole number of kSlots-block stretches.
+        // chain-bound inner loop; the prefetch runs kSlots blocks ahead, so a row is gated one row early.  A row
+        // (1024 blocks) is a whole number of kUnroll-block stretches.
         for (uint32_t base = 0; base < trips; base += 1024) {
             gate((base >> 10) + 1, (uint64_t)(base + 1024) * 64 < len);
             const uint32_t iend = min(base + 1024, trips);
-            for (uint32_t i = base; i < iend; i += kSlots) blocks(i);
+            for (uint32_t i = base; i < iend; i += kUnroll) blocks(i);
         }
     } else {
         // Sender side: one flat loop (measured 1.027x faster per block than the nested form).
-        for (uint32_t i = 0; i < trips; i += kSlots) blocks(i);
+        for (uint32_t i = 0; i < trips; i += kUnroll) {
+            blocks(i);
+#ifdef SKY_MD5_TRACE
+            const uint32_t done = i + kUnroll;
+            if (trace && lane == 0 && done % kTraceEvery == 0 && done / kTraceEvery <= kTraceStamps)
+                trace->s[done / kTraceEvery - 1] = Md5TraceStamp{trace_globaltimer(), trace_clock(), wait_cycles};
+#endif
+        }
     }
+#ifdef SKY_MD5_TRACE
+    if (trace && lane == 0) {
+        trace->t1 = trace_globaltimer();
+        trace->c1 = trace_clock();
+        trace->wait = wait_cycles;
+        trace->blocks = trips;
+        trace->stamps = min(trips / kTraceEvery, (uint32_t)kTraceStamps);
+    }
+#endif
     cp_async_wait<0>();
     st = fin;
     uint32_t xxh = 0;

@@ -15,7 +15,9 @@
 // the frame length.  The high-ratio compressor (lz4hc.cuh, SKY_F_HC) claims, loads and places its blocks through the
 // same frame.cuh helpers.
 //
-// The two roles never wait on each other: digest lanes and compressors each read their own input from HBM.
+// Digest lanes and compressors each read their own input from HBM, and a digest lane never waits for a compressor.  A
+// compressor CTA that shares an SM with a running chain steps aside while the LZ4 work is projected to finish well before
+// the chain (wait_for_chain), so the chain keeps its SM's issue slots.
 //
 // Host side: sky_ctx owns every stream, event and buffer through move-only owners that release them in their destructors:
 // per slot a kernel stream, batch metadata, the receiver's and the E2EE arrays and (optionally) input / output slabs for
@@ -58,7 +60,9 @@ constexpr int kThreads = kWarps * 32;
 #endif
 constexpr int kRing = kParsers + SKY_RING_EXTRA;       // segment slots between the prober and the parsers
 constexpr int kMd5WarpsPerCta = 4;        // digest CTAs run 4 MD5 groups (one per SM sub-partition), see sky_fused_kernel
-constexpr uint32_t kRingBytes = SKY_MD5_SLOTS * 2048;  // MD5 staging ring: slots x 64 B x 32 lanes
+constexpr uint32_t kRingBytes = SKY_MD5_SLOTS * 2048;  // sender's MD5 staging ring: slots x 64 B x 32 lanes
+constexpr int kDecMd5Slots = 4;           // the receiver's MD5 ring (its copies are of bytes the decode warps just wrote, in L2)
+constexpr uint32_t kDecRingBytes = kDecMd5Slots * 2048;
 constexpr int kCtasPerSm = 2;             // fused kernel: 2 x ~110 KiB of shared memory per SM
 constexpr uint64_t kMaxChunkBlocks = 1ull << 21;  // 64 KiB blocks = 128 GiB per chunk: md5_warp counts 64-byte blocks in 32 bits
 
@@ -75,6 +79,7 @@ struct Ctl {
     uint64_t data;                      // frame offset of the block's first data byte
     uint32_t size;                      // the block's data bytes in the frame (kBlkChk only)
     PendingChecksum pend;               // kBlkChk: the CTA's last compressed block until kSumWarp hashes it
+    uint64_t t0;                        // %clock64 when the CTA started (wait_for_chain)
 };
 constexpr uint32_t kInOff = 0;
 constexpr uint32_t kTabOff = kInOff + kInBytes;
@@ -87,6 +92,65 @@ static_assert(kSmemBytes <= 232448 / 2 - 1024, "two CTAs per SM need <= 112.5 Ki
 static_assert(kEntries % 128 == 0, "SKY_LZ4_ENTRIES must be a multiple of 128");
 static_assert(kMd5WarpsPerCta * kRingBytes <= kInBytes, "the MD5 rings live in the block buffer of a digest CTA");
 static_assert(sizeof(SegSlot) % 16 == 0 && sizeof(SegRec) == 16 && sizeof(SegPlan) == 16, "layout");
+
+#ifdef SKY_MD5_TRACE
+// Diagnostic build only (see md5.cuh): thread 0 of every fused-kernel CTA that compresses records its SM, when it
+// started, when it claimed its first and last block and when it found the claim counter exhausted.
+constexpr int kTraceCtas = 1024;
+struct CtaTrace {
+    uint32_t smid, digest, claims, pad;
+    uint64_t entry, first, last, exhausted;
+};
+__device__ CtaTrace g_cta_trace[kTraceCtas];
+#endif
+
+// ---- compressors step aside for the MD5 chains of their SM ----------------------------------------------------------
+// A digest CTA in a launch that also compresses publishes, in its SM's word behind the claim counter, the %clock64 by which
+// its warp 0's chains would end at the chain's floor rate.  Before each block claim, thread 0 of a compressing CTA on that
+// SM reads the word: while the chains run and the claims so far project the LZ4 work to end well before them, the CTA
+// waits instead of claiming, since its probers and parsers would take issue slots from the chain (§4.1: an MD5 chain ran
+// 3.5 % slower per block while the compressor beside it claimed blocks).  Where compressing is the longer stage (config 3)
+// the projection says so and nothing waits.  The wait ends on the clock, so it needs nothing to clear it, and a CTA waits
+// only between blocks, holding no OFF-chain word: every block before the ones it would claim was claimed by a CTA that is
+// running, so the OFF chain stays deadlock-free (frame.cuh).
+#ifndef SKY_CHAIN_WAIT
+#define SKY_CHAIN_WAIT 1
+#endif
+constexpr bool kChainWait = SKY_CHAIN_WAIT != 0;        // 0: compressors never wait (tools/build_variants.py no_chain_wait)
+constexpr uint32_t kSmWords = 256;                      // per-SM words (%smid < kSmWords) after the counters' first 64 bytes
+constexpr uint32_t kCountersBytes = 64 + kSmWords * 8;  // cleared before every launch
+constexpr uint64_t kChainCyclesPerBlock = 780;          // 12.16 cycles x 64 steps: the static schedule (under load it runs slower)
+__device__ __forceinline__ uint64_t *sm_chain_end(const Params &p) { return reinterpret_cast<uint64_t *>(p.counters + 16); }
+__device__ __forceinline__ uint32_t sm_id() {
+    uint32_t s;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+    return s;
+}
+// One thread of a digest CTA, as its chains start.  md5_order lists each group's longest chunk first.
+__device__ __forceinline__ void publish_chain_end(const Params &p) {
+    uint64_t blocks = 0;
+    for (uint32_t g = blockIdx.x; g < p.n_groups; g += p.n_md5_ctas * kMd5WarpsPerCta) blocks += p.chunks[p.md5_order[g * 32]].len >> 6;
+    const uint32_t s = sm_id();
+    if (s < kSmWords)
+        atomicMax(reinterpret_cast<unsigned long long *>(sm_chain_end(p) + s), (unsigned long long)(clock64() + blocks * kChainCyclesPerBlock));
+}
+// Thread 0 of a compressing CTA, before it claims a block; t0 = its %clock64 at start.
+__device__ __forceinline__ void wait_for_chain(const Params &p, uint64_t t0) {
+    const uint32_t s = sm_id();
+    if (s >= kSmWords) return;
+    uint64_t end;
+    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(end) : "l"(sm_chain_end(p) + s) : "memory");
+    const uint32_t total = p.rows * p.n_chunks;
+    for (;;) {
+        const uint64_t now = clock64();
+        const uint32_t w = ld_relaxed32(p.counters);
+        // the chain is done, too few claims to project from (1/64 of the blocks), or none left
+        if (now >= end || w <= total / 64 || w >= total) return;
+        const float left = (float)(now - t0) * ((float)(total - w) / (float)w);  // the rest at the claims' rate so far
+        if (1.25f * left >= (float)(end - now)) return;  // not clearly ahead of the chain: keep compressing
+        __nanosleep(10000);
+    }
+}
 
 // named-barrier token between the two prober warps: the releaser arrives, the waiter syncs (ids 1 and 2, 64 threads)
 template <int kId>
@@ -118,6 +182,14 @@ __device__ __forceinline__ void fused_body(const Params &p) {
     asm volatile("" : "+r"(smem_s));   // compiler re-derives it (S2UR SR_CgaCtaId + ULEA) at the top of every prober batch
 
     const bool do_md5 = (p.flags & SKY_F_MD5) != 0, do_lz4 = (p.flags & SKY_F_LZ4) != 0;
+#ifdef SKY_MD5_TRACE
+    CtaTrace tr{};
+    if (warp == 0 && lane == 0) {
+        tr.smid = trace_smid();
+        tr.digest = do_md5 && blockIdx.x < p.n_md5_ctas;
+        tr.entry = trace_globaltimer();
+    }
+#endif
     if (warp == 0 && lane == 0) {
         mbar_init(&ctl->in_full, 1);
         for (int i = 0; i < kRing; i++) {
@@ -125,12 +197,14 @@ __device__ __forceinline__ void fused_body(const Params &p) {
             mbar_init(&ctl->empty[i], 1);
         }
         ctl->claim = 0;
+        ctl->t0 = clock64();
         if constexpr (kBlkChk) ctl->pend.data = nullptr;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
     if (do_md5 && blockIdx.x < p.n_md5_ctas) {
+        if (kChainWait && do_lz4 && warp == kWarps - 1 && lane == 0) publish_chain_end(p);  // (an idle warp: warps 0-3 carry the chains)
         if (warp < kMd5WarpsPerCta) {
             for (uint32_t g = warp * p.n_md5_ctas + blockIdx.x; g < p.n_groups; g += p.n_md5_ctas * kMd5WarpsPerCta) {
                 const uint32_t c = p.md5_order[g * 32 + lane];
@@ -142,7 +216,11 @@ __device__ __forceinline__ void fused_body(const Params &p) {
                     len = p.chunks[c].len;
                 }
                 const uint32_t x = md5_warp<kXxh>(reinterpret_cast<uint32_t *>(in + warp * kRingBytes), src, len, active,
-                                                  p.md5_out + (size_t)(active ? c : 0) * 16, lane);
+                                                  p.md5_out + (size_t)(active ? c : 0) * 16, lane
+#ifdef SKY_MD5_TRACE
+                                                  , Md5NoGate(), g < kTraceGroups ? &g_md5_trace[g] : nullptr
+#endif
+                );
                 if constexpr (kXxh) {
                     if (active) p.xxh_out[c] = x;
                 }
@@ -164,9 +242,20 @@ __device__ __forceinline__ void fused_body(const Params &p) {
     for (uint32_t it = 0;; it++) {
         BlockDesc *dsc = &ctl->desc[it & 1];
         if (warp == 0 && lane == 0) {
+            if (kChainWait && p.n_md5_ctas) wait_for_chain(p, ctl->t0);  // (the CTA's other threads wait at the barrier below)
             claim_block(p, dsc);
             ctl->block_end_seq = 0xffffffffu;
             ctl->nseg = 0;
+#ifdef SKY_MD5_TRACE
+            const uint64_t t = trace_globaltimer();
+            if (dsc->valid) {
+                if (tr.claims++ == 0) tr.first = t;
+                tr.last = t;
+            } else {
+                tr.exhausted = t;
+                if (blockIdx.x < kTraceCtas) g_cta_trace[blockIdx.x] = tr;
+            }
+#endif
         }
         __syncthreads();  // (also: every warp is done with the previous block's buffer, records and plan)
         if (!dsc->valid) {
@@ -474,8 +563,8 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
                 len = p.chunks[c].raw_len;
                 gate.flags = p.blk_done + p.chunks[c].blk_base;
             }
-            const uint32_t x = md5_warp<true>(reinterpret_cast<uint32_t *>(smem + warp * kRingBytes), src, len, active,
-                                              p.md5_out + (size_t)(active ? c : 0) * 16, lane, gate);
+            const uint32_t x = md5_warp<true, DecRowGate, kDecMd5Slots>(reinterpret_cast<uint32_t *>(smem + warp * kDecRingBytes), src, len,
+                                                                        active, p.md5_out + (size_t)(active ? c : 0) * 16, lane, gate);
             // every row has passed the gate, so no decode warp reads or writes the status any more: settle a block failure
             // into its code (lz4dec.cuh); a content checksum mismatch only replaces ok
             if (active) {
@@ -742,7 +831,7 @@ static int build_slot(sky_ctx *ctx, Slot &s, bool slabs) {
     CK(ctx, m.outlen.alloc(nc));
     CK(ctx, m.md5.alloc(nc * 16));
     CK(ctx, cudaMalloc(m.xxh.put(), nc * sizeof(uint32_t)));
-    CK(ctx, cudaMalloc(m.counters.put(), 64));
+    CK(ctx, cudaMalloc(m.counters.put(), kCountersBytes));
     CK(ctx, cudaMalloc(m.scratch.put(), (size_t)ctx->sm_count * kCtasPerSm * kScratchBytes));
     if (slabs) {
         cudaError_t e = cudaMalloc(s.d_in.put(), ctx->in_cap);
@@ -1131,7 +1220,7 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
         CK(ctx, cudaEventRecord(s.ev_h2d, meta_st));  // input (enqueued earlier on meta_st) + metadata have landed
         CK(ctx, cudaStreamWaitEvent(st, s.ev_h2d, 0));
     }
-    CK(ctx, cudaMemsetAsync(m.counters, 0, 64, st));
+    CK(ctx, cudaMemsetAsync(m.counters, 0, kCountersBytes, st));  // the claim counter and the per-SM chain words
     memset(m.outlen.h, 0, n * sizeof(uint64_t));  // host-side clear (mapped memory; the slot is idle here)
     memset(m.md5.h, 0, (size_t)n * 16);
 
@@ -1433,7 +1522,7 @@ static int launch_decode(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, con
     CK(ctx, cudaEventRecord(s.ev_k0, st));
     sky_frame_index_kernel<<<(n + 127) / 128, 128, 0, st>>>(p);
     CK(ctx, cudaGetLastError());
-    sky_decode_kernel<<<ctx->sm_count, 512, kMd5WarpsPerCta * kRingBytes, st>>>(p);
+    sky_decode_kernel<<<ctx->sm_count, 512, kMd5WarpsPerCta * kDecRingBytes, st>>>(p);
     CK(ctx, cudaGetLastError());
     CK(ctx, cudaEventRecord(s.ev_k1, st));
     ctx->launches += 2;
@@ -1559,5 +1648,23 @@ int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64
 }
 
 uint64_t sky_launch_count(const sky_ctx *ctx) { return ctx ? ctx->launches : 0; }
+
+#ifdef SKY_MD5_TRACE
+// Diagnostic build only, not part of the ABI: copies the trace records of the last fused launches on `device` to the host
+// (sizes in bytes, as tools/md5_trace.py lays them out) and clears them.
+SKY_API int sky_md5_trace_fetch(int device, void *md5, uint64_t md5_bytes, void *ctas, uint64_t cta_bytes) {
+    if (md5_bytes != sizeof(sky::g_md5_trace) || cta_bytes != sizeof(sky::g_cta_trace)) return SKY_E_INVALID;
+    if (cudaSetDevice(device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess ||
+        cudaMemcpyFromSymbol(md5, sky::g_md5_trace, md5_bytes) != cudaSuccess ||
+        cudaMemcpyFromSymbol(ctas, sky::g_cta_trace, cta_bytes) != cudaSuccess)
+        return SKY_E_CUDA;
+    static const char zero[sizeof(sky::g_md5_trace)] = {};
+    static_assert(sizeof(sky::g_md5_trace) >= sizeof(sky::g_cta_trace), "one zero buffer clears both");
+    if (cudaMemcpyToSymbol(sky::g_md5_trace, zero, md5_bytes) != cudaSuccess ||
+        cudaMemcpyToSymbol(sky::g_cta_trace, zero, cta_bytes) != cudaSuccess)
+        return SKY_E_CUDA;
+    return SKY_OK;
+}
+#endif
 
 }  // extern "C"

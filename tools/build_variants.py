@@ -11,6 +11,12 @@ VARIANTS = {
     "pa10_r3": {"SKY_PARSERS": 10, "SKY_RING_EXTRA": 3},
     "pa12_r2": {"SKY_PARSERS": 12, "SKY_RING_EXTRA": 2},  # the default build
     "pa13_r1": {"SKY_PARSERS": 13, "SKY_RING_EXTRA": 1},
+    # diagnostic: the sender's MD5 warps and compressor CTAs stamp their timeline (tools/md5_trace.py reads it)
+    "md5_trace": {"SKY_MD5_TRACE": 1},
+    # the sender's MD5 ring half as deep (the default is 8): copies staged 4 blocks ahead of the chain
+    "md5_slots4": {"SKY_MD5_SLOTS": 4},
+    # compressors never step aside for the MD5 chains of their SM
+    "no_chain_wait": {"SKY_CHAIN_WAIT": 0},
 }
 
 if __name__ == "__main__":
