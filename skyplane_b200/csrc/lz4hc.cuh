@@ -19,6 +19,10 @@
 //   place  : the OFF chain gives the block's frame offset (place_block), and all warps copy it there.
 // Claim, load, placement and write-out are frame.cuh's, shared with sky_fused_kernel.
 //
+// Optimal parse (SKY_F_OPTIMAL, sky_hc_opt{,_bc,_linked,_linked_bc}_kernel): between search and emission every warp
+// parses its own 2 KiB segment of the block by the bytes the sequences cost (opt_segment, the twin's
+// hc_compress_block_opt), and warp 0 then emits the matches the segments chose instead of the lazy parse's.
+//
 // Linked blocks (SKY_F_LINKED, sky_hc_linked{,_bc}_kernel): block j >= 1 of a chunk also sees the chunk's 64 KiB before it
 // (the twin's hc_compress_block_linked).  Shared memory has no room for that window, so it stays where it is:
 //   window bytes : read from the chunk in global memory (d.src - 65536, L2-resident) by load32x / load8x, which read shared
@@ -79,10 +83,82 @@ __device__ __forceinline__ uint32_t load8x(uint32_t in_s, const uint8_t *src, in
     return x >= 0 ? lds8(in_s + (uint32_t)x) : (uint32_t)__ldg(src + x);
 }
 
+// ---- optimal parse (SKY_F_OPTIMAL): the twin's hc_compress_block_opt, whose header states the rule.  Each warp parses its
+// own kHcOptSeg-byte segments (one per warp in a 64 KiB block) in the shared memory the search leaves free:
+//   len_s (chains, first half): the search's u8 length per position; a window's lengths are cleared once its forward pass
+//          is done, and the backtrace writes there the length of every match the parse starts (255 + u16 length in the
+//          next two bytes for a long match), which is what warp 0 emits from;
+//   dec_s (chains, second half, and the head table's first byte at p = 65536): per position, the length of the match
+//          that ends there in its kept state, 0 = reached by a literal.  A window [a, e] writes it at a < p <= e only, so
+//          a warp writes and reads dec_s in (s0, s1] alone: the next warp's segment starts at s1 but never writes there.
+// Forward pass: lane j holds the state of position p + j, packed as cost << 17 | run << 5 | last, so that the twin's
+// lexicographic (cost, run, last) order is the u32 order.  Lane 0's state is final; lane 1 takes the literal from p, lanes
+// 4 .. min(len(p), e - p) the match of their own length; then the states move down one lane.
+constexpr uint32_t kHcOptSeg = 2048;
+static_assert(kHcOptSeg * kHcWarps == kBlock, "one parse segment per warp of a whole block");
+static_assert(kHcOptSeg < 4096 && kHcNice <= 32, "a state packs its run in 12 bits and its last match in 5");
+constexpr uint32_t kOptCost = 17, kOptLong = 255;
+template <bool kLinked>
+__device__ __forceinline__ void opt_segment(uint32_t in_s, const uint8_t *src, uint32_t len_s, uint32_t dec_s, const uint16_t *g_off,
+                                            uint32_t s0, uint32_t s1, uint32_t mflimit, uint32_t matchlimit, unsigned lane) {
+    const uint32_t need = lane == 1u ? 0u : lane >= kMinMatch ? lane : 0xffu;  // lane 1: the literal; 4..31: match length
+    const uint32_t mstep = ((3u + (lane >= kMinMatch + 15u ? 1u : 0u)) << kOptCost) | lane;
+    for (uint32_t a = s0; a < s1;) {
+        uint32_t e = s1;  // the first long position at or after a
+        for (uint32_t b = a; b < s1; b += 32) {
+            const uint32_t x = b + lane;
+            const unsigned m = __ballot_sync(kFull, x < s1 && x <= mflimit && s1 - x >= kHcNice && lds8(len_s + x) == kHcNice);
+            if (m) {
+                e = b + (uint32_t)__ffs(m) - 1u;
+                break;
+            }
+        }
+        uint32_t st = lane == 0 ? 0u : 0xffffffffu;
+        for (uint32_t p = a; p < e; p++) {
+            const uint32_t k0 = __shfl_sync(kFull, st, 0);
+            if (lane == 0 && p != a) sts8(dec_s + p, k0 & 31u);  // (the backtrace stops at a)
+            const uint32_t len = p <= mflimit ? lds8(len_s + p) : 0u;
+            const uint32_t run = ((k0 >> 5) & 0xfffu) + 1u;
+            const uint32_t bump = (run + 240u) * 0xFEFEFEFFu <= 0x01010101u ? 2u : 1u;  // a length byte more at 15, 270, ...
+            const uint32_t cand = lane == 1u ? (((k0 >> kOptCost) + bump) << kOptCost) | (run << 5) : (k0 & ~((1u << kOptCost) - 1u)) + mstep;
+            if (need <= min(len, e - p)) st = min(st, cand);
+            st = __shfl_down_sync(kFull, st, 1);
+            if (lane == 31) st = 0xffffffffu;
+        }
+        if (lane == 0 && e != a) sts8(dec_s + e, st & 31u);
+        for (uint32_t x = a + lane; x < e; x += 32) sts8(len_s + x, 0u);
+        __syncwarp();
+        for (uint32_t q = e; q > a;) {  // backtrace: the nearest position at or before q reached by a match, 32 at a time
+            const uint32_t v = lane < q - a ? lds8(dec_s + q - lane) : 0u;
+            const unsigned m = __ballot_sync(kFull, v != 0u);
+            if (!m) {
+                q = q - a > 32u ? q - 32u : a;
+                continue;
+            }
+            const uint32_t f = (uint32_t)__ffs(m) - 1u, ml = __shfl_sync(kFull, v, f);
+            q -= f + ml;
+            if (lane == 0) sts8(len_s + q, ml);
+        }
+        if (e == s1) break;
+        const uint32_t cand = e - __ldcg(g_off + e), lim = min(matchlimit, s1) - e;
+        uint32_t ml;
+        if constexpr (kLinked) ml = extend_coop([in_s, src](uint32_t x) { return load32x(in_s, src, (int32_t)x); }, e, cand, kHcNice, lim, lane);
+        else ml = extend_coop_s(in_s, e, cand, kHcNice, lim, lane);
+        if (lane == 0) {
+            sts8(len_s + e, kOptLong);
+            sts8(len_s + e + 1u, ml & 0xffu);
+            sts8(len_s + e + 2u, ml >> 8);
+        }
+        __syncwarp();
+        a = e + ml;
+    }
+}
+
 // kHcDepth: chain candidates walked per position, hc_depth(level).  kBlkChk (SKY_F_BLOCK_CHECKSUM): every block gets its
 // checksum (block_checksum), hashed from the frame by warp 1 during the next block's chain step, which only warp 0 works
 // on (or before the CTA exits).  kLinked (SKY_F_LINKED): blocks after a chunk's first match into its previous 64 KiB.
-template <uint32_t kHcDepth, bool kBlkChk, bool kLinked = false>
+// kOpt (SKY_F_OPTIMAL): every warp parses its segment optimally (opt_segment) before warp 0 emits the chosen matches.
+template <uint32_t kHcDepth, bool kBlkChk, bool kLinked = false, bool kOpt = false>
 __device__ __forceinline__ void hc_body(const Params &p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -228,6 +304,12 @@ __device__ __forceinline__ void hc_body(const Params &p) {
             for (uint32_t k = tid; k < (mflimit + 16u) / 16u; k += kHcThreads) dst4[k] = __ldcg(src4 + k);
         }
         __syncthreads();
+        if constexpr (kOpt) {  // ------------------------------------------- optimal parse, one segment per warp
+            if (has_matches)
+                for (uint32_t s0 = warp * kHcOptSeg; s0 < L; s0 += kHcWarps * kHcOptSeg)
+                    opt_segment<kLinked>(in_s, d.src, chain_s, chain_s + kBlock, g_off, s0, min(s0 + kHcOptSeg, L), mflimit, matchlimit, lane);
+            __syncthreads();
+        }
         // ---------------------------------------------------------------- lazy parse + emission (warp 0), then placement
         if (warp == 0) {
             uint32_t op = 0, anchor = 0;
@@ -237,16 +319,23 @@ __device__ __forceinline__ void hc_body(const Params &p) {
                     if (cur <= mflimit) {
                         const uint32_t x = cur + lane;
                         const uint32_t len = x <= mflimit ? lds8(chain_s + x) : 0u;
-                        uint32_t nxt = __shfl_down_sync(kFull, len, 1);
-                        if (lane == 31) nxt = x + 1u <= mflimit ? lds8(chain_s + x + 1u) : 0u;
-                        const unsigned take = __ballot_sync(kFull, len >= kMinMatch && nxt <= len);
+                        unsigned take;
+                        if constexpr (kOpt) {  // the matches the optimal parse chose
+                            take = __ballot_sync(kFull, len != 0u);
+                        } else {
+                            uint32_t nxt = __shfl_down_sync(kFull, len, 1);
+                            if (lane == 31) nxt = x + 1u <= mflimit ? lds8(chain_s + x + 1u) : 0u;
+                            take = __ballot_sync(kFull, len >= kMinMatch && nxt <= len);
+                        }
                         if (!take) {
                             cur += 32;
                             continue;
                         }
                         const uint32_t f = (uint32_t)__ffs(take) - 1u, pos = cur + f;
                         uint32_t ml = __shfl_sync(kFull, len, f);
-                        if (ml == kHcNice) {
+                        if constexpr (kOpt) {
+                            if (ml == kOptLong) ml = lds8(chain_s + pos + 1u) | (lds8(chain_s + pos + 2u) << 8);
+                        } else if (ml == kHcNice) {
                             const uint32_t cand = pos - __ldcg(g_off + pos);
                             if constexpr (kLinked) {
                                 const uint8_t *src = d.src;
@@ -299,5 +388,14 @@ template <uint32_t kHcDepth>
 __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_linked_kernel(const Params p) { hc_body<kHcDepth, false, true>(p); }
 template <uint32_t kHcDepth>
 __global__ void __launch_bounds__(kHcThreads, 1) sky_hc_linked_bc_kernel(const Params p) { hc_body<kHcDepth, true, true>(p); }
+// SKY_F_OPTIMAL: the four with the optimal parse (same shared memory and scratch as their lazy counterparts).
+template <uint32_t kHcDepth>
+__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_opt_kernel(const Params p) { hc_body<kHcDepth, false, false, true>(p); }
+template <uint32_t kHcDepth>
+__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_opt_bc_kernel(const Params p) { hc_body<kHcDepth, true, false, true>(p); }
+template <uint32_t kHcDepth>
+__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_opt_linked_kernel(const Params p) { hc_body<kHcDepth, false, true, true>(p); }
+template <uint32_t kHcDepth>
+__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_opt_linked_bc_kernel(const Params p) { hc_body<kHcDepth, true, true, true>(p); }
 
 }  // namespace sky

@@ -720,6 +720,25 @@ static const HcKernel kHcLinkedBcKernels[] = {sky_hc_linked_bc_kernel<hc_depth(3
                                               sky_hc_linked_bc_kernel<hc_depth(9)>};
 static_assert(sizeof(kHcLinkedKernels) == sizeof(kHcKernels) && sizeof(kHcLinkedBcKernels) == sizeof(kHcKernels),
               "one linked HC kernel, with and without block checksums, per level");
+// ... and all four with the optimal parse (SKY_F_OPTIMAL)
+static const HcKernel kHcOptKernels[] = {sky_hc_opt_kernel<hc_depth(3)>, sky_hc_opt_kernel<hc_depth(4)>, sky_hc_opt_kernel<hc_depth(5)>,
+                                         sky_hc_opt_kernel<hc_depth(6)>, sky_hc_opt_kernel<hc_depth(7)>, sky_hc_opt_kernel<hc_depth(8)>,
+                                         sky_hc_opt_kernel<hc_depth(9)>};
+static const HcKernel kHcOptBcKernels[] = {sky_hc_opt_bc_kernel<hc_depth(3)>, sky_hc_opt_bc_kernel<hc_depth(4)>,
+                                           sky_hc_opt_bc_kernel<hc_depth(5)>, sky_hc_opt_bc_kernel<hc_depth(6)>,
+                                           sky_hc_opt_bc_kernel<hc_depth(7)>, sky_hc_opt_bc_kernel<hc_depth(8)>,
+                                           sky_hc_opt_bc_kernel<hc_depth(9)>};
+static const HcKernel kHcOptLinkedKernels[] = {sky_hc_opt_linked_kernel<hc_depth(3)>, sky_hc_opt_linked_kernel<hc_depth(4)>,
+                                               sky_hc_opt_linked_kernel<hc_depth(5)>, sky_hc_opt_linked_kernel<hc_depth(6)>,
+                                               sky_hc_opt_linked_kernel<hc_depth(7)>, sky_hc_opt_linked_kernel<hc_depth(8)>,
+                                               sky_hc_opt_linked_kernel<hc_depth(9)>};
+static const HcKernel kHcOptLinkedBcKernels[] = {sky_hc_opt_linked_bc_kernel<hc_depth(3)>, sky_hc_opt_linked_bc_kernel<hc_depth(4)>,
+                                                 sky_hc_opt_linked_bc_kernel<hc_depth(5)>, sky_hc_opt_linked_bc_kernel<hc_depth(6)>,
+                                                 sky_hc_opt_linked_bc_kernel<hc_depth(7)>, sky_hc_opt_linked_bc_kernel<hc_depth(8)>,
+                                                 sky_hc_opt_linked_bc_kernel<hc_depth(9)>};
+static_assert(sizeof(kHcOptKernels) == sizeof(kHcKernels) && sizeof(kHcOptBcKernels) == sizeof(kHcKernels) &&
+              sizeof(kHcOptLinkedKernels) == sizeof(kHcKernels) && sizeof(kHcOptLinkedBcKernels) == sizeof(kHcKernels),
+              "one optimal-parse HC kernel of each kind per level");
 constexpr uint32_t kHcLevelShift = 8, kHcLevelMask = 0xfu << kHcLevelShift;  // SKY_F_HC_LEVEL's field in `flags`
 static_assert(SKY_F_HC_LEVEL(1) == (SKY_F_HC | (1u << kHcLevelShift)), "the level field of include/skychunk.h");
 // The level a batch's flags select: the level field, or kHcDefaultLevel when it is 0.
@@ -975,6 +994,7 @@ uint32_t sky_kernel_config(int what) {
     case 5: return kHcHashBits;
     case 6: return kHcNice;
     case 7: return (uint32_t)kHcMaxLevel;
+    case 8: return kHcOptSeg;
     default: return 0;
     }
 }
@@ -1017,6 +1037,14 @@ int sky_ctx_create(int device, uint64_t max_batch_bytes, uint32_t max_chunks, ui
     for (const HcKernel k : kHcLinkedKernels)
         if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcLinkedSmemBytes);
     for (const HcKernel k : kHcLinkedBcKernels)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcLinkedSmemBytes);
+    for (const HcKernel k : kHcOptKernels)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
+    for (const HcKernel k : kHcOptBcKernels)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
+    for (const HcKernel k : kHcOptLinkedKernels)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcLinkedSmemBytes);
+    for (const HcKernel k : kHcOptLinkedBcKernels)
         if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcLinkedSmemBytes);
     if (e != cudaSuccess) {
         g_err = ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (this build carries sm_90a code only)";
@@ -1137,11 +1165,11 @@ static uint32_t fill_md5_order(uint32_t *order, uint32_t n, const uint64_t *len)
 
 // SKY_F_HC selects how frames are made, SKY_F_CHECKSUM / SKY_F_BLOCK_CHECKSUM add to the frame and SKY_F_VERIFY checks
 // it, so each needs SKY_F_LZ4, or no stage bit at all (= LZ4 + MD5).  A level field needs SKY_F_HC and a level in kHcMinLevel .. kHcMaxLevel.
-// SKY_F_LINKED needs SKY_F_HC: only the high-ratio compressor links blocks.
+// SKY_F_LINKED and SKY_F_OPTIMAL need SKY_F_HC: only the high-ratio compressor links blocks and parses optimally.
 static bool frame_flags_valid(uint32_t flags) {
     if ((flags & kHcLevelMask) && (!(flags & SKY_F_HC) || hc_level(flags) < kHcMinLevel || hc_level(flags) > kHcMaxLevel))
         return false;
-    if ((flags & SKY_F_LINKED) && !(flags & SKY_F_HC)) return false;
+    if ((flags & (SKY_F_LINKED | SKY_F_OPTIMAL)) && !(flags & SKY_F_HC)) return false;
     return !(flags & (SKY_F_HC | SKY_F_CHECKSUM | SKY_F_BLOCK_CHECKSUM | SKY_F_VERIFY)) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5;
 }
 // Bytes a chunk's frame may take: SKY_F_CHECKSUM adds the 4-byte content checksum behind the EndMark,
@@ -1262,10 +1290,12 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
         }
         p.scratch = h.scratch;
         const int lv = hc_level(flags) - kHcMinLevel;
+        const bool opt = (flags & SKY_F_OPTIMAL) != 0;
         if (flags & SKY_F_LINKED)
-            (bc ? kHcLinkedBcKernels : kHcLinkedKernels)[lv]<<<ctx->sm_count, kHcThreads, kHcLinkedSmemBytes, st>>>(p);
+            (opt ? (bc ? kHcOptLinkedBcKernels : kHcOptLinkedKernels) : (bc ? kHcLinkedBcKernels : kHcLinkedKernels))[lv]<<<
+                ctx->sm_count, kHcThreads, kHcLinkedSmemBytes, st>>>(p);
         else
-            (bc ? kHcBcKernels : kHcKernels)[lv]<<<ctx->sm_count, kHcThreads, kHcSmemBytes, st>>>(p);
+            (opt ? (bc ? kHcOptBcKernels : kHcOptKernels) : (bc ? kHcBcKernels : kHcKernels))[lv]<<<ctx->sm_count, kHcThreads, kHcSmemBytes, st>>>(p);
         CK(ctx, cudaGetLastError());
         if (md5) CK(ctx, cudaStreamWaitEvent(st, h.ev_join, 0));
     } else {

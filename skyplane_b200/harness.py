@@ -63,13 +63,15 @@ def run_stream(
     block_checksum: bool = False,
     verify_frames: bool = False,
     block_linked: bool = False,
+    optimal_parse: bool = False,
 ) -> Dict:
     """Stream ``n_requests`` chunk requests (recycling ``pool_files`` by hard link) through the operator.
 
     The first ``warmup_requests`` completions are not timed (worker start-up: CUDA context, pinned staging).
-    ``high_ratio``, ``content_checksum``, ``compression_level``, ``block_checksum``, ``verify_frames`` and ``block_linked`` are
-    handed to the operator (GatewayCompressHash's high-ratio frames, frames with LZ4's content checksum, the high-ratio level,
-    frames with LZ4's block checksums, the GPU's check of every frame, linked blocks) when set.
+    ``high_ratio``, ``content_checksum``, ``compression_level``, ``block_checksum``, ``verify_frames``, ``block_linked`` and
+    ``optimal_parse`` are handed to the operator (GatewayCompressHash's high-ratio frames, frames with LZ4's content
+    checksum, the high-ratio level, frames with LZ4's block checksums, the GPU's check of every frame, linked blocks, the
+    optimal parse) when set.
     Returns {"wall_s", "bytes", "records": [{chunk_id, pool_index, md5, raw_len, frame_path}], "status": {...},
     "frame_verify": {chunk_id: status of every chunk whose frame failed the check}}.
     """
@@ -87,6 +89,7 @@ def run_stream(
         **({"block_checksum": True} if block_checksum else {}),
         **({"verify_frames": True} if verify_frames else {}),
         **({"block_linked": True} if block_linked else {}),
+        **({"optimal_parse": True} if optimal_parse else {}),
     )
     op.start_workers()
     records: List[Dict] = []

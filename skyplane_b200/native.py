@@ -18,6 +18,7 @@ SKY_E_INVALID, SKY_E_NOGPU, SKY_E_CUDA, SKY_E_CAPACITY, SKY_E_BUSY, SKY_E_TICKET
 F_LZ4, F_MD5, F_E2EE, F_HC, F_CHECKSUM, F_BLOCK_CHECKSUM = 1, 2, 16, 32, 64, 128
 F_VERIFY = 1 << 12  # every frame is checked against its chunk on the GPU; one that fails is sent as its stored-block frame
 F_LINKED = 1 << 13  # with F_HC only: linked blocks (python-lz4's block_linked), matches may reach into the previous 64 KiB
+F_OPTIMAL = 1 << 14  # with F_HC only: the optimal parse (sequences chosen by their cost in bytes) over the same match search
 CHECKSUM_BYTES = 4  # F_CHECKSUM: the content checksum (u32le XXH32) behind the EndMark; F_BLOCK_CHECKSUM: as many per block
 BLOCK_BYTES = 65536
 # SKY_F_HC_LEVEL(l): the high-ratio level l (3..9: 2**(l - 1) chain candidates per position) in bits 8..11 of the flags;
@@ -151,7 +152,8 @@ def kernel_config() -> dict:
     L = lib()
     return {"lz4_entries": L.sky_kernel_config(0), "warps": L.sky_kernel_config(1), "seg_slots": L.sky_kernel_config(2),
             "max_step_log": L.sky_kernel_config(3), "hc_depth": L.sky_kernel_config(4), "hc_hash_bits": L.sky_kernel_config(5),
-            "hc_nice": L.sky_kernel_config(6), "hc_max_level": L.sky_kernel_config(7)}
+            "hc_nice": L.sky_kernel_config(6), "hc_max_level": L.sky_kernel_config(7),
+            "hc_opt_seg": L.sky_kernel_config(8)}
 
 
 def hc_depth(level: int) -> int:
@@ -198,7 +200,8 @@ def frame_need(n: int, checksum: bool = False, block_checksum: bool = False) -> 
 
 
 _DECODE_ONLY_SUBMIT = ((F_HC, "F_HC"), (HC_LEVEL_MASK, "a high-ratio level"), (F_CHECKSUM, "F_CHECKSUM"),
-                       (F_BLOCK_CHECKSUM, "F_BLOCK_CHECKSUM"), (F_VERIFY, "F_VERIFY"), (F_LINKED, "F_LINKED"))
+                       (F_BLOCK_CHECKSUM, "F_BLOCK_CHECKSUM"), (F_VERIFY, "F_VERIFY"), (F_LINKED, "F_LINKED"),
+                       (F_OPTIMAL, "F_OPTIMAL"))
 
 
 def check_decode_flags(flags: int) -> int:

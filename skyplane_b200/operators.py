@@ -142,6 +142,7 @@ class GatewayCompressHash(GatewayOperator):
         block_checksum: bool = False,
         verify_frames: bool = False,
         block_linked: bool = False,
+        optimal_parse: bool = False,
     ):
         """use_compression / e2ee_key_bytes: GatewaySender's arguments of the same name (gateway_operator.py:154-168):
         ``use_compression=False`` digests the chunk and lets it pass through uncompressed (``is_compressed=False``);
@@ -162,6 +163,9 @@ class GatewayCompressHash(GatewayOperator):
         block_linked: python-lz4's argument of the same name, for the high-ratio parse (``ChunkStage.launch(linked=True)``): a
         match may reach up to 65535 bytes back into the chunk's previous block, which saves bytes on text.  The default stays
         independent blocks.  Needs ``high_ratio`` or a ``compression_level`` of 3..9.
+        optimal_parse: the high-ratio frames with the optimal parse (``ChunkStage.launch(optimal=True)``): the same match
+        search, sequences chosen by their cost in bytes, so fewer bytes at the same level for more GPU time.  The frame
+        format and receiver stay the same.  Off by default.  Needs ``high_ratio`` or a ``compression_level`` of 3..9.
         sink: ``callable(worker_id) -> socket``, called once in each worker.  With a sink the worker sends every payload
         straight from the pinned staging slot (``wire.send_results``: WireProtocolHeader + payload, no intermediate bytes
         object, no frame file) -- the tail of ``GatewaySender.process`` (gateway_operator.py:367-402)."""
@@ -185,6 +189,9 @@ class GatewayCompressHash(GatewayOperator):
         if block_linked and not hc_bits:
             raise ValueError("block_linked is a mode of the high-ratio compressor: it needs high_ratio or a compression_level of 3..9")
         self.block_linked = bool(block_linked)
+        if optimal_parse and not hc_bits:
+            raise ValueError("optimal_parse is a parse of the high-ratio compressor: it needs high_ratio or a compression_level of 3..9")
+        self.optimal_parse = bool(optimal_parse)
         self.compression_level = compression_level
         self.e2ee_key_bytes = e2ee_key_bytes
         self.sink = sink
@@ -339,6 +346,8 @@ class GatewayCompressHash(GatewayOperator):
             opts["verify"] = True
         if self.block_linked:
             opts["linked"] = True
+        if self.optimal_parse:
+            opts["optimal"] = True
         stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None, **opts)
         return True
 

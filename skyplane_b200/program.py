@@ -37,6 +37,7 @@ def _compress_hash(op: Dict, kw: Dict) -> GatewayOperator:
         block_checksum=op.get("block_checksum", False),
         verify_frames=op.get("verify_frames", False),
         block_linked=op.get("block_linked", False),
+        optimal_parse=op.get("optimal_parse", False),
         max_batch_chunks=op.get("max_batch_chunks", 64),
         max_batch_bytes=op.get("max_batch_bytes", 512 << 20),
         n_gpus=op.get("num_gpus"),

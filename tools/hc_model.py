@@ -1,6 +1,7 @@
 """Python face of tools/lz4hc_model.c, the sequential CPU twin of the high-ratio (SKY_F_HC) block compressor (development /
 test tool, not product code).  frame(data) is the LZ4 frame the GPU stage must emit byte for byte with SKY_F_HC, and
-frame(data, linked=True) the one it emits with SKY_F_HC | SKY_F_LINKED."""
+frame(data, linked=True) the one it emits with SKY_F_HC | SKY_F_LINKED, and frame(data, optimal=True) the one it emits with
+SKY_F_HC | SKY_F_OPTIMAL (parse segments of OPT_SEG bytes, sky_kernel_config(8))."""
 from __future__ import annotations
 
 import ctypes
@@ -40,22 +41,30 @@ def lib():
         _lib.hc_compress_block.restype = ctypes.c_uint32
         _lib.hc_compress_block_linked.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_char_p, ctypes.POINTER(Opts)]
         _lib.hc_compress_block_linked.restype = ctypes.c_uint32
+        _lib.hc_compress_block_opt.argtypes = [ctypes.c_void_p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_char_p,
+                                               ctypes.POINTER(Opts)]
+        _lib.hc_compress_block_opt.restype = ctypes.c_uint32
     return _lib
 
 
 WINDOW = 65536  # linked: source bytes before a block (after the chunk's first) that its matches may reach
+OPT_SEG = 2048  # the kernel's optimal-parse segment (sky_kernel_config(8))
 
 
-def blocks(data: bytes, o: Opts, linked: bool = False):
+def blocks(data: bytes, o: Opts, linked: bool = False, optimal: bool = False, seg: int = OPT_SEG):
     """-> list of (compressed size or 0 when stored raw, block bytes as they appear in the frame).  linked: blocks after
-    the first see the previous 64 KiB of the chunk (hc_compress_block_linked)."""
+    the first see the previous 64 KiB of the chunk (hc_compress_block_linked).  optimal: the optimal parse with segments
+    of `seg` bytes, 0 = one per block (hc_compress_block_opt)."""
     L = lib()
     buf = ctypes.create_string_buffer(65536 + 4096)
-    src = ctypes.create_string_buffer(bytes(data), len(data)) if linked else None
+    src = ctypes.create_string_buffer(bytes(data), len(data)) if (linked or optimal) else None
     out = []
     for pos in range(0, len(data), 65536):
         blk = data[pos:pos + 65536]
-        if linked:
+        if optimal:
+            c = L.hc_compress_block_opt(ctypes.addressof(src) + pos, len(blk), min(pos, WINDOW) if linked else 0, seg, buf,
+                                        ctypes.byref(o))
+        elif linked:
             c = L.hc_compress_block_linked(ctypes.addressof(src) + pos, len(blk), min(pos, WINDOW), buf, ctypes.byref(o))
         else:
             c = L.hc_compress_block(blk, len(blk), buf, ctypes.byref(o))
@@ -63,8 +72,9 @@ def blocks(data: bytes, o: Opts, linked: bool = False):
     return out
 
 
-def frame(data: bytes, o: Opts | None = None, block_checksum: bool = False, linked: bool = False) -> bytes:
-    return tile_model.assemble(len(data), blocks(data, o or kernel_opts(), linked), block_checksum, linked)
+def frame(data: bytes, o: Opts | None = None, block_checksum: bool = False, linked: bool = False, optimal: bool = False,
+          seg: int = OPT_SEG) -> bytes:
+    return tile_model.assemble(len(data), blocks(data, o or kernel_opts(), linked, optimal, seg), block_checksum, linked)
 
 
 def liblz4_frame(data: bytes, level: int, linked: bool = False, content_checksum: bool = False, block_checksum: bool = False) -> bytes:

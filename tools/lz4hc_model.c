@@ -26,6 +26,31 @@
  *              candidate uses no depth.  Candidates are compared against the chunk's source bytes, so a match may run
  *              from the previous block into this one.  Block j depends on source bytes only, never on block j-1's output.
  *              With hist = 0 it is hc_compress_block, byte for byte.
+ *   optimal    (SKY_F_OPTIMAL, hc_compress_block_opt) the same chains and search (blen, boff); only the parse differs.
+ *              It picks the sequences of least byte cost among these candidates, independent or linked:
+ *     segments   positions split into segments of `seg` bytes [s0, s1) (seg = 0: one segment per block).  No match
+ *                crosses its segment's end, and a segment's parse depends on nothing before it: it starts closed (no
+ *                open literal run) at s0, which is what lets the kernel parse the segments in parallel.
+ *     long       a position p <= mflimit with blen(p) = nice and s1 - p >= nice is long.  The first long position e at or
+ *                after the window start a ends the window [a, e]: the parse reaches e by the cheapest path from a and
+ *                takes the match at e extended with the same candidate up to min(matchlimit, s1), as the lazy parse
+ *                extends it (liblz4's optimal parse takes a match past its sufficient length the same way).  The next
+ *                window starts closed at its end.  Without a long position the window is [a, s1].
+ *     candidates from p in a window [a, e]: the literal p -> p + 1, and a match of every length ml = 4 .. min(blen(p), e - p)
+ *                at boff(p) (so lengths up to nice - 1: no long position lies inside a window).
+ *     cost       the bytes a sequence takes: 1 + litext(ll) + ll + 2 + mlext(ml - 4), where a length field's extension
+ *                bytes are litext(x) = mlext(x) = x >= 15 ? 1 + (x - 15) / 255 : 0 (the final literals' token is the same
+ *                in every parse).  A literal run is carried as liblz4 carries it: each position keeps one state (cost,
+ *                run, last) -- cost of the cheapest path to it including its open run's literal bytes, that run's length,
+ *                and the length of the match that ends there (0: reached by a literal).  A literal adds
+ *                lit(run + 1) - lit(run), lit(x) = x + litext(x); a match adds 3 + mlext(ml - 4) and closes the run.
+ *                One kept run per position is what makes this an approximation: two paths of equal cost with different
+ *                runs may differ by one extension byte later.
+ *     ties       positions are relaxed in order, each one's state final before it is relaxed; a state is replaced only
+ *                by a lexicographically smaller (cost, run, last).  The order of relaxation therefore does not matter.
+ *     backtrace  from e (or s1) back to a through `last`; the matches it passes, and the long match, are the window's.
+ *     emission   the chosen matches in position order across all segments with one anchor, so a literal run that
+ *                crosses a segment's start becomes one sequence; the final literals [anchor, L).  Stored raw as above.
  *
  * Build: gcc -O2 -shared -fPIC -o tools/bin/liblz4hc.so tools/lz4hc_model.c
  */
@@ -59,9 +84,63 @@ static uint32_t emit(uint8_t *out, uint32_t op, const uint8_t *src, uint32_t anc
 
 #define WINDOW 65535  /* the largest offset */
 
+/* literal run ll: its bytes plus its length field's extension bytes (the token is counted with the sequence) */
+static uint32_t lit_price(uint32_t ll) { return ll + (ll >= 15 ? 1 + (ll - 15) / 255 : 0); }
+/* a match of ml bytes after its literal run: token, offset, match length extension bytes */
+static uint32_t match_price(uint32_t ml) { return 3 + (ml - MINMATCH >= 15 ? 1 + (ml - MINMATCH - 15) / 255 : 0); }
+
+/* Optimal parse (hc_compress_block_opt): writes sel[p] = the length of the match the parse starts at p, 0 elsewhere.
+   See the header comment for the rule; blen / boff are the search's (blen[p] = 0 below 4, p > mflimit: 0). */
+static void opt_parse(const uint8_t *src, uint32_t L, uint32_t seg, uint32_t nice, const uint32_t *blen, const uint32_t *boff,
+                      uint32_t *sel) {
+    const uint32_t mflimit = L - MFLIMIT, matchlimit = L - LASTLITERALS;
+    uint32_t *price = malloc((L + 1) * sizeof(uint32_t)), *run = malloc((L + 1) * sizeof(uint32_t)),
+             *last = malloc((L + 1) * sizeof(uint32_t));
+    if (seg == 0) seg = L;
+    for (uint32_t s0 = 0; s0 < L; s0 += seg) {
+        const uint32_t s1 = L - s0 < seg ? L : s0 + seg;  /* the segment's end: no match crosses it */
+        uint32_t a = s0;
+        while (a < s1) {
+            uint32_t e = a;  /* the window ends at the first long position, else at the segment's end */
+            while (e < s1 && !(e <= mflimit && blen[e] == nice && s1 - e >= nice)) e++;
+            price[a] = 0; run[a] = 0; last[a] = 0;
+            for (uint32_t q = a + 1; q <= e; q++) price[q] = UINT32_MAX;
+            for (uint32_t p = a; p < e; p++) {  /* p's state is final: relax the literal and every match from p */
+                const uint32_t ll = run[p] + 1, lp = price[p] - lit_price(run[p]) + lit_price(ll);
+                uint32_t cp = lp, cr = ll, cm = 0;
+                /* (cost, run, last) is compared lexicographically; the smaller replaces */
+                if (cp < price[p + 1] || (cp == price[p + 1] && (cr < run[p + 1] || (cr == run[p + 1] && cm < last[p + 1])))) {
+                    price[p + 1] = cp; run[p + 1] = cr; last[p + 1] = cm;
+                }
+                const uint32_t maxml = blen[p] < e - p ? blen[p] : e - p;
+                for (uint32_t ml = MINMATCH; ml <= maxml; ml++) {
+                    const uint32_t q = p + ml;
+                    cp = price[p] + match_price(ml); cr = 0; cm = ml;
+                    if (cp < price[q] || (cp == price[q] && (cr < run[q] || (cr == run[q] && cm < last[q])))) {
+                        price[q] = cp; run[q] = cr; last[q] = cm;
+                    }
+                }
+            }
+            for (uint32_t q = a; q < e; q++) sel[q] = 0;
+            for (uint32_t q = e; q > a;) {  /* backtrace */
+                const uint32_t m = last[q];
+                if (m) { q -= m; sel[q] = m; } else q--;
+            }
+            if (e == s1) break;
+            uint32_t ml = nice;  /* the long match at e, extended with the same candidate, clipped to the segment */
+            const uint32_t lim = (matchlimit < s1 ? matchlimit : s1) - e;
+            while (ml < lim && src[e + ml] == src[(int64_t)e - boff[e] + ml]) ml++;
+            sel[e] = ml;
+            a = e + ml;
+        }
+    }
+    free(price); free(run); free(last);
+}
+
 /* returns the compressed size, or 0 if the block does not shrink (store raw); out capacity >= L + 2048.
-   src[-hist .. -1] are visible (linked blocks); hist = 0: an independent block. */
-static uint32_t compress_block(const uint8_t *src, uint32_t L, uint32_t hist, uint8_t *out, const hc_opts *o) {
+   src[-hist .. -1] are visible (linked blocks); hist = 0: an independent block.  opt: the optimal parse with segments of
+   `seg` bytes (0: one segment), else the lazy parse. */
+static uint32_t compress_block(const uint8_t *src, uint32_t L, uint32_t hist, int opt, uint32_t seg, uint8_t *out, const hc_opts *o) {
     uint32_t op = 0, anchor = 0;
     if (L >= MFLIMIT + 1) {
         const uint32_t mflimit = L - MFLIMIT, matchlimit = L - LASTLITERALS;
@@ -69,7 +148,7 @@ static uint32_t compress_block(const uint8_t *src, uint32_t L, uint32_t hist, ui
         const int64_t none = INT64_MIN;
         int64_t *head = malloc(nh * sizeof(int64_t));
         int64_t *chain = (int64_t *)malloc((hist + mflimit + 1) * sizeof(int64_t)) + hist;  /* chain[p], p = -hist .. mflimit */
-        uint32_t *blen = calloc(mflimit + 2, sizeof(uint32_t)), *boff = calloc(mflimit + 2, sizeof(uint32_t));
+        uint32_t *blen = calloc(L + 1, sizeof(uint32_t)), *boff = calloc(L + 1, sizeof(uint32_t));
         for (uint32_t h = 0; h < nh; h++) head[h] = none;
         for (int64_t p = -(int64_t)hist; p <= (int64_t)mflimit; p++) {
             const uint32_t h = (rd32(src + p) * 2654435761u) >> (32 - o->hash_bits);
@@ -88,16 +167,28 @@ static uint32_t compress_block(const uint8_t *src, uint32_t L, uint32_t hist, ui
             }
             if (best >= MINMATCH) { blen[p] = best; boff[p] = bo; }
         }
-        uint32_t p = 0;
-        while (p <= mflimit) {
-            const uint32_t ml0 = blen[p];
-            if (ml0 < MINMATCH || blen[p + 1] > ml0) { p++; continue; }  /* (blen[mflimit + 1] = 0) */
-            uint32_t ml = ml0;
-            const uint32_t off = boff[p];
-            if (ml == nice) while (p + ml < matchlimit && src[p + ml] == src[(int64_t)p - off + ml]) ml++;
-            op = emit(out, op, src, anchor, p - anchor, ml, off);
-            p += ml;
-            anchor = p;
+        if (opt) {
+            uint32_t *sel = calloc(L + 1, sizeof(uint32_t));
+            opt_parse(src, L, seg, nice, blen, boff, sel);
+            for (uint32_t p = 0; p <= mflimit;) {
+                if (!sel[p]) { p++; continue; }
+                op = emit(out, op, src, anchor, p - anchor, sel[p], boff[p]);
+                p += sel[p];
+                anchor = p;
+            }
+            free(sel);
+        } else {
+            uint32_t p = 0;
+            while (p <= mflimit) {
+                const uint32_t ml0 = blen[p];
+                if (ml0 < MINMATCH || blen[p + 1] > ml0) { p++; continue; }  /* (blen[mflimit + 1] = 0) */
+                uint32_t ml = ml0;
+                const uint32_t off = boff[p];
+                if (ml == nice) while (p + ml < matchlimit && src[p + ml] == src[(int64_t)p - off + ml]) ml++;
+                op = emit(out, op, src, anchor, p - anchor, ml, off);
+                p += ml;
+                anchor = p;
+            }
         }
         free(head); free(chain - hist); free(blen); free(boff);
     }
@@ -106,10 +197,16 @@ static uint32_t compress_block(const uint8_t *src, uint32_t L, uint32_t hist, ui
 }
 
 uint32_t hc_compress_block(const uint8_t *src, uint32_t L, uint8_t *out, const hc_opts *o) {
-    return compress_block(src, L, 0, out, o);
+    return compress_block(src, L, 0, 0, 0, out, o);
 }
 
 /* a block of a linked chunk: src[-hist .. -1] are the chunk's bytes before it (hist = 0 for block 0, else 65536) */
 uint32_t hc_compress_block_linked(const uint8_t *src, uint32_t L, uint32_t hist, uint8_t *out, const hc_opts *o) {
-    return compress_block(src, L, hist, out, o);
+    return compress_block(src, L, hist, 0, 0, out, o);
+}
+
+/* the optimal parse (SKY_F_OPTIMAL) of an independent (hist = 0) or linked block, with parse segments of `seg` bytes
+   (0: the whole block is one segment) */
+uint32_t hc_compress_block_opt(const uint8_t *src, uint32_t L, uint32_t hist, uint32_t seg, uint8_t *out, const hc_opts *o) {
+    return compress_block(src, L, hist, 1, seg, out, o);
 }

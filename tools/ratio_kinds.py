@@ -2,7 +2,8 @@
 """Compression ratio of the kernel's parse (its sequential CPU twin, tools/lz4_tile_model.c) on data kinds beyond the bench's
 Silesia-like set, next to liblz4's: linked blocks (what the reference emits) and independent blocks (what any block-parallel
 compressor is limited to), plus the twin's linked-block mode (blocks after a chunk's first match into the previous 64 KiB
-window), the high-ratio parse (SKY_F_HC, its twin tools/lz4hc_model.c) and its linked blocks (SKY_F_LINKED).  Development tool: CPU only, reads files that happen to be installed in the build container."""
+window), the high-ratio parse (SKY_F_HC, its twin tools/lz4hc_model.c), its linked blocks (SKY_F_LINKED) and its optimal parse
+(SKY_F_OPTIMAL, independent and linked).  Development tool: CPU only, reads files that happen to be installed in the build container."""
 import glob
 import json
 import os
@@ -60,13 +61,17 @@ if __name__ == "__main__":
         ours_linked = len(tm.frame(d, linked=True))
         hc = len(hm.frame(d))
         hc_linked = len(hm.frame(d, linked=True))
+        hc_opt = len(hm.frame(d, optimal=True))
+        hc_linked_opt = len(hm.frame(d, linked=True, optimal=True))
         linked = len(ref.lz4f_compress(d))
         indep = len(oracle.lz4f_compress_indep(d)) if hasattr(oracle, "lz4f_compress_indep") else None
         row = {"data": name, "bytes": raw, "kernel_parse_ratio": round(raw / ours, 4), "liblz4_linked_ratio": round(raw / linked, 4),
                "vs_reference": round(linked / ours, 4), "linked_parse_ratio": round(raw / ours_linked, 4),
                "linked_vs_reference": round(linked / ours_linked, 4), "hc_parse_ratio": round(raw / hc, 4), "hc_vs_reference": round(linked / hc, 4),
                "hc_linked_ratio": round(raw / hc_linked, 4), "hc_linked_vs_hc": round(hc / hc_linked, 4),
-               "hc_linked_vs_reference": round(linked / hc_linked, 4)}
+               "hc_linked_vs_reference": round(linked / hc_linked, 4), "hc_opt_ratio": round(raw / hc_opt, 4),
+               "hc_opt_vs_hc": round(hc / hc_opt, 4), "hc_linked_opt_ratio": round(raw / hc_linked_opt, 4),
+               "hc_linked_opt_vs_hc_linked": round(hc_linked / hc_linked_opt, 4)}
         if indep:
             row["liblz4_independent_blocks_ratio"] = round(raw / indep, 4)
             row["vs_liblz4_independent"] = round(indep / ours, 4)

@@ -7,7 +7,8 @@ hc3-checksum .. hc9-checksum (SKY_F_HC_LEVEL(3..9): the high-ratio mode at that 
 block-checksum, block-checksum-checksum, hc-block-checksum, hc-block-checksum-checksum and hc3-block-checksum ..
 hc9-block-checksum (SKY_F_BLOCK_CHECKSUM: the same frames with LZ4's block checksums, alone or with the content checksum);
 hc-linked, hc3-linked .. hc9-linked and their -checksum / -block-checksum forms (SKY_F_LINKED: the high-ratio frames with
-linked blocks).
+linked blocks); hc-opt, hc3-opt .. hc9-opt and hc-linked-opt, hc3-linked-opt .. hc9-linked-opt (SKY_F_OPTIMAL: the same
+frames from the optimal parse).
 --decode-from liblz4[-linked][-checksums] times the receiver on liblz4's level-0 frames made on the host from the same
 input: independent or linked blocks, without checksums or with block and content checksums.
 --ref-ratio adds the reference's ratio (liblz4 level 0, linked blocks) on the distinct chunks; --liblz4-level9 times liblz4
@@ -195,6 +196,9 @@ def main():
     for k in [k for k in FL if k.startswith("hc") and k != "hc-lz4"]:  # hc5-checksum -> hc5-linked-checksum
         head, _, tail = k.partition("-")
         FL[f"{head}-linked" + (f"-{tail}" if tail else "")] = FL[k] | native.F_LINKED
+    for k in [k for k in FL if k.split("-")[0] in [f"hc{lv}" for lv in range(native.HC_MIN_LEVEL, native.HC_MAX_LEVEL + 1)] + ["hc"]
+              and k.removeprefix(k.split("-")[0]) in ("", "-linked")]:  # hc5 -> hc5-opt, hc5-linked -> hc5-linked-opt
+        FL[f"{k}-opt"] = FL[k] | native.F_OPTIMAL
     FL.update({"block-checksum": native.F_BLOCK_CHECKSUM, "block-checksum-checksum": native.F_BLOCK_CHECKSUM | native.F_CHECKSUM,
                "hc-block-checksum": native.F_HC | native.F_BLOCK_CHECKSUM,
                "hc-block-checksum-checksum": native.F_HC | native.F_BLOCK_CHECKSUM | native.F_CHECKSUM})
