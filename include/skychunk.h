@@ -119,6 +119,19 @@ extern "C" {
  * SKY_F_LINKED) for 3.8 % more GPU time.  Without SKY_F_HC, or with SKY_F_MD5 alone, it is SKY_E_INVALID.  For sky_verify_device it names the
  * compressor that made the frames, as SKY_F_HC does.  sky_decode does not take it: a frame states its own format. */
 #define SKY_F_OPTIMAL 16384u
+/* pass-through of incompressible chunks (sky_submit only): chunk i is sent as itself when its final frame -- after
+ * SKY_F_VERIFY's repair, if that is set -- is not smaller than the chunk (frame_len[i] >= src_len[i]); every other chunk is
+ * sent as its frame, byte for byte the frame the batch makes without this flag.  The frames are made as always; only what
+ * comes back changes.  For a chunk that passes through: without SKY_F_E2EE out_len[i] = 0 and dst[i] is not written (as
+ * with SKY_F_MD5 alone, the caller forwards its own input bytes, and nothing is copied back for it); with SKY_F_E2EE dst[i]
+ * holds the SecretBox of the chunk's own bytes and out_len[i] = src_len[i] + SKY_BOX_OVERHEAD.  The digests always come
+ * back, and SKY_F_VERIFY's statuses too.  Such a ticket is completed by sky_wait_ex only, whose compressed[i] says which
+ * payload each chunk got; sky_wait and sky_wait_verify return SKY_E_INVALID and leave it waitable.  It needs SKY_F_LZ4 (or
+ * no stage bit) and combines with SKY_F_HC / SKY_F_HC_LEVEL / SKY_F_LINKED / SKY_F_OPTIMAL, SKY_F_E2EE and SKY_F_VERIFY.
+ * With SKY_F_MD5 alone, SKY_F_CHECKSUM or SKY_F_BLOCK_CHECKSUM (a raw payload cannot carry the LZ4 checksums) it is
+ * SKY_E_INVALID, as it is in sky_process_device, sky_verify_device and sky_decode: the receiver takes the chunks that pass
+ * through as it takes SKY_F_MD5's payloads. */
+#define SKY_F_PASSTHROUGH 32768u
 
 typedef struct sky_ctx sky_ctx;
 
@@ -171,6 +184,12 @@ SKY_API int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *
  * made it, whose payload is now the stored-block frame.  verify != NULL needs a ticket submitted with SKY_F_VERIFY
  * (SKY_E_INVALID otherwise, and the ticket stays un-waited); sky_wait also completes such a ticket. */
 SKY_API int sky_wait_verify(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, float *kernel_ms);
+/* sky_wait_verify, plus compressed[n] (required): per chunk 1 when its payload is a frame (or the SecretBox of a frame), 0
+ * when it is the chunk itself (or the SecretBox of the chunk) -- WireProtocolHeader.is_compressed.  It completes any
+ * ticket: without SKY_F_PASSTHROUGH compressed[i] is 1 exactly when the ticket has SKY_F_LZ4.  verify follows
+ * sky_wait_verify's rules. */
+SKY_API int sky_wait_ex(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, uint8_t *compressed,
+                        float *kernel_ms);
 SKY_API int sky_set_e2ee_key(sky_ctx *ctx, const uint8_t *key32);
 SKY_API uint64_t sky_box_bound(uint64_t n); /* sky_frame_bound(n) + SKY_BOX_OVERHEAD */
 
@@ -201,6 +220,8 @@ SKY_API int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, cons
  *     ... | SKY_F_E2EE                SecretBox of the frame          SKY_F_E2EE (with or without the two bits)
  *     SKY_F_MD5 (`compress: false`)   the chunk's own bytes           SKY_F_MD5
  *     SKY_F_MD5 | SKY_F_E2EE          SecretBox of the chunk          SKY_F_MD5 | SKY_F_E2EE
+ *     ... | SKY_F_PASSTHROUGH         per chunk, one of the rows      per chunk, by sky_wait_ex's compressed[i]:
+ *                                     above (frame or chunk)          the frames' row or the chunks' row
  *
  * SKY_F_E2EE: the payloads are sealed boxes, whose tags are checked and which are opened on the device first (status
  * SKY_D_AUTH for a forged / truncated box, whose bytes are never returned; SKY_E_NOKEY without a key).

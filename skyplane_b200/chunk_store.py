@@ -2,7 +2,9 @@
 
 Layout the stage relies on:
   <chunk_dir>/<chunk_id>.chunk       the chunk's bytes (tmpfs in production, compute/server.py:341)
-  <chunk_dir>/<chunk_id>.chunk.lz4   ours: the LZ4 frame produced by / delivered to the H100 stage
+  <chunk_dir>/<chunk_id>.chunk.lz4   ours: the LZ4 frame produced by / delivered to the H100 stage (or its SecretBox)
+  <chunk_dir>/<chunk_id>.chunk.box   ours: the SecretBox of a chunk of a compressed transfer that was sent as itself
+                                     (skip_incompressible); such a chunk sent unsealed has no payload file of its own
 Operators report state changes with ``log_chunk_state``; the records travel through ``chunk_status_queue`` to
 whoever plays the gateway API's role (gateway_daemon_api.py:89-155).
 """
@@ -20,6 +22,7 @@ from skyplane_b200.gateway_queue import GatewayQueue
 
 CHUNK_SUFFIX = ".chunk"
 FRAME_SUFFIX = ".chunk.lz4"
+BOX_SUFFIX = ".chunk.box"
 
 
 def _utc_stamp() -> str:
@@ -37,7 +40,7 @@ class ChunkStore:
 
     def _purge_leftovers(self) -> None:
         """A gateway always starts with an empty chunk directory (chunk_store.py:21-24)."""
-        for pattern in ("*" + CHUNK_SUFFIX, "*" + FRAME_SUFFIX):
+        for pattern in ("*" + CHUNK_SUFFIX, "*" + FRAME_SUFFIX, "*" + BOX_SUFFIX):
             for leftover in self.chunk_dir.glob(pattern):
                 leftover.unlink()
 
@@ -129,6 +132,19 @@ class ChunkStore:
 
     def get_compressed_file_path(self, chunk_id: str) -> Path:
         return self.chunk_dir / (chunk_id + FRAME_SUFFIX)
+
+    def get_box_file_path(self, chunk_id: str) -> Path:
+        return self.chunk_dir / (chunk_id + BOX_SUFFIX)
+
+    def wire_payload(self, chunk_id: str) -> Tuple[Path, bool]:
+        """What a sender of a compressed transfer puts on the wire for a chunk the H100 stage has handled (INTEGRATION §2):
+        -> (payload file, WireProtocolHeader.is_compressed).  ``.chunk.lz4`` is a frame or the box of a frame; ``.chunk.box``
+        is the box of a chunk sent as itself; with neither, ``<chunk_id>.chunk`` itself goes, uncompressed.  (With
+        ``compress: false`` every payload is uncompressed, whatever its file.)"""
+        for path, compressed in ((self.get_compressed_file_path(chunk_id), True), (self.get_box_file_path(chunk_id), False)):
+            if path.exists():
+                return path, compressed
+        return self.get_chunk_file_path(chunk_id), False
 
     def remaining_bytes(self) -> int:
         try:

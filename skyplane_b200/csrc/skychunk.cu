@@ -621,14 +621,25 @@ __global__ void __launch_bounds__(512, 1) sky_decode_kernel(const DecParams p) {
 // side knows every length before it starts, so its descriptors are built on the host, see launch_open).
 // seal: msg = the chunk's frame (or, without LZ4, its raw bytes), box = box_base + (frame offset in the frame slab) + 64*i + 8,
 // so that box + 40 is 16-byte aligned; the nonce is copied in, out_len becomes the box length.
-__global__ void sky_box_setup_kernel(BoxChunk *bc, uint64_t *blk_base, const ChunkDesc *desc, uint32_t n, uint64_t *out_len,
-                                     const uint8_t *frame_slab, uint8_t *box_slab, const uint8_t *nonces, int use_frames) {
+// kPass (SKY_F_PASSTHROUGH): msg = the frame where it is smaller than the chunk, otherwise the chunk's own bytes, and
+// pass[i] = 1 for a chunk sealed raw.
+template <bool kPass>
+__device__ __forceinline__ void box_setup_body(BoxChunk *bc, uint64_t *blk_base, const ChunkDesc *desc, uint32_t n, uint64_t *out_len,
+                                               const uint8_t *frame_slab, uint8_t *box_slab, const uint8_t *nonces, int use_frames,
+                                               uint8_t *pass) {
     for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
         const ChunkDesc d = desc[i];
         BoxChunk b;
         b.box = box_slab + (d.dst - frame_slab) + 64ull * i + 8;
-        b.msg = use_frames ? d.dst : d.src;
-        b.len = use_frames ? out_len[i] : d.len;
+        if (kPass) {
+            const bool raw = out_len[i] >= d.len;
+            b.msg = raw ? d.src : d.dst;
+            b.len = raw ? d.len : out_len[i];
+            pass[i] = raw;
+        } else {
+            b.msg = use_frames ? d.dst : d.src;
+            b.len = use_frames ? out_len[i] : d.len;
+        }
         for (int k = 0; k < 24; k++) b.box[k] = nonces[24ull * i + k];
         bc[i] = b;
         out_len[i] = b.len + kBoxOverhead;
@@ -642,6 +653,24 @@ __global__ void sky_box_setup_kernel(BoxChunk *bc, uint64_t *blk_base, const Chu
         }
         blk_base[n] = acc;
     }
+}
+__global__ void sky_box_setup_kernel(BoxChunk *bc, uint64_t *blk_base, const ChunkDesc *desc, uint32_t n, uint64_t *out_len,
+                                     const uint8_t *frame_slab, uint8_t *box_slab, const uint8_t *nonces, int use_frames) {
+    box_setup_body<false>(bc, blk_base, desc, n, out_len, frame_slab, box_slab, nonces, use_frames, nullptr);
+}
+__global__ void sky_box_setup_pass_kernel(BoxChunk *bc, uint64_t *blk_base, const ChunkDesc *desc, uint32_t n, uint64_t *out_len,
+                                          const uint8_t *frame_slab, uint8_t *box_slab, const uint8_t *nonces, uint8_t *pass) {
+    box_setup_body<true>(bc, blk_base, desc, n, out_len, frame_slab, box_slab, nonces, 1, pass);
+}
+
+// SKY_F_PASSTHROUGH without E2EE: a chunk whose final frame is not smaller than the chunk is sent as itself.  pass[i] = 1
+// and out_len[i] = 0 for it, so that nothing is copied back (the caller holds the chunk's bytes).
+__global__ void sky_passthrough_kernel(const ChunkDesc *desc, uint64_t *out_len, uint8_t *pass, uint32_t n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const bool raw = out_len[i] >= desc[i].len;
+    pass[i] = raw;
+    if (raw) out_len[i] = 0;
 }
 
 }  // namespace sky
@@ -689,6 +718,7 @@ struct BatchMeta {  // one batch's descriptors and results (the receiver uses th
     // device->host copies sit in a copy-engine queue behind multi-GiB frame copies
     Mapped<uint64_t> outlen;
     Mapped<uint8_t> md5;
+    Mapped<uint8_t> pass;     // SKY_F_PASSTHROUGH: per chunk 1 when its payload is the chunk itself, not its frame
     DevMem<uint32_t> xxh;     // per chunk XXH32 of the input (SKY_F_CHECKSUM)
     DevMem<uint32_t> counters;
     DevMem<uint8_t> scratch;  // compress scratch: kScratchBytes per CTA of the grid (kernels of different slots overlap)
@@ -849,6 +879,7 @@ static int build_slot(sky_ctx *ctx, Slot &s, bool slabs) {
     CK(ctx, cudaMalloc(m.d_chain.put(), nc * sizeof(uint64_t)));
     CK(ctx, m.outlen.alloc(nc));
     CK(ctx, m.md5.alloc(nc * 16));
+    CK(ctx, m.pass.alloc(nc));
     CK(ctx, cudaMalloc(m.xxh.put(), nc * sizeof(uint32_t)));
     CK(ctx, cudaMalloc(m.counters.put(), kCountersBytes));
     CK(ctx, cudaMalloc(m.scratch.put(), (size_t)ctx->sm_count * kCtasPerSm * kScratchBytes));
@@ -1104,11 +1135,16 @@ int sky_set_e2ee_key(sky_ctx *ctx, const uint8_t *key32) {
     return SKY_OK;
 }
 
-// Seal the batch's frames (or raw chunks) on `st` after the fused kernel: setup -> keys -> xor -> tag.
+// Seal the batch's frames (or raw chunks; with SKY_F_PASSTHROUGH each chunk's frame or the chunk, whichever is smaller) on
+// `st` after the fused kernel: setup -> keys -> xor -> tag.
 static int launch_seal(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, uint8_t *d_dst, uint32_t flags) {
     const int use_frames = (flags & SKY_F_LZ4) ? 1 : 0;
     BoxArrays &b = s.box;
-    sky_box_setup_kernel<<<1, 256, 0, st>>>(b.d_chunks, b.d_blk_base, s.meta.d_desc, n, s.meta.outlen.d, d_dst, b.d_box, b.d_nonce, use_frames);
+    if (flags & SKY_F_PASSTHROUGH)
+        sky_box_setup_pass_kernel<<<1, 256, 0, st>>>(b.d_chunks, b.d_blk_base, s.meta.d_desc, n, s.meta.outlen.d, d_dst, b.d_box, b.d_nonce,
+                                                     s.meta.pass.d);
+    else
+        sky_box_setup_kernel<<<1, 256, 0, st>>>(b.d_chunks, b.d_blk_base, s.meta.d_desc, n, s.meta.outlen.d, d_dst, b.d_box, b.d_nonce, use_frames);
     CK(ctx, cudaGetLastError());
     sky_box_keys_kernel<<<(n + 63) / 64, 64, 0, st>>>(b.d_chunks, n, ctx->d_key, b.d_sub);
     CK(ctx, cudaGetLastError());
@@ -1166,11 +1202,15 @@ static uint32_t fill_md5_order(uint32_t *order, uint32_t n, const uint64_t *len)
 // SKY_F_HC selects how frames are made, SKY_F_CHECKSUM / SKY_F_BLOCK_CHECKSUM add to the frame and SKY_F_VERIFY checks
 // it, so each needs SKY_F_LZ4, or no stage bit at all (= LZ4 + MD5).  A level field needs SKY_F_HC and a level in kHcMinLevel .. kHcMaxLevel.
 // SKY_F_LINKED and SKY_F_OPTIMAL need SKY_F_HC: only the high-ratio compressor links blocks and parses optimally.
+// SKY_F_PASSTHROUGH chooses between a frame and the chunk, so it needs SKY_F_LZ4 too, and a raw payload cannot carry the
+// LZ4 checksums SKY_F_CHECKSUM / SKY_F_BLOCK_CHECKSUM ask for.
 static bool frame_flags_valid(uint32_t flags) {
     if ((flags & kHcLevelMask) && (!(flags & SKY_F_HC) || hc_level(flags) < kHcMinLevel || hc_level(flags) > kHcMaxLevel))
         return false;
     if ((flags & (SKY_F_LINKED | SKY_F_OPTIMAL)) && !(flags & SKY_F_HC)) return false;
-    return !(flags & (SKY_F_HC | SKY_F_CHECKSUM | SKY_F_BLOCK_CHECKSUM | SKY_F_VERIFY)) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5;
+    if ((flags & SKY_F_PASSTHROUGH) && (flags & (SKY_F_CHECKSUM | SKY_F_BLOCK_CHECKSUM))) return false;
+    return !(flags & (SKY_F_HC | SKY_F_CHECKSUM | SKY_F_BLOCK_CHECKSUM | SKY_F_VERIFY | SKY_F_PASSTHROUGH)) ||
+           (flags & (SKY_F_LZ4 | SKY_F_MD5)) != SKY_F_MD5;
 }
 // Bytes a chunk's frame may take: SKY_F_CHECKSUM adds the 4-byte content checksum behind the EndMark,
 // SKY_F_BLOCK_CHECKSUM 4 bytes behind every block.
@@ -1317,6 +1357,10 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
     if (flags & SKY_F_E2EE) {
         rc = launch_seal(ctx, s, st, n, d_dst, flags);
         if (rc != SKY_OK) return rc;
+    } else if (flags & SKY_F_PASSTHROUGH) {  // every frame is final: mark the chunks that go as themselves
+        sky_passthrough_kernel<<<(n + 127) / 128, 128, 0, st>>>(m.d_desc, m.outlen.d, m.pass.d, n);
+        CK(ctx, cudaGetLastError());
+        ctx->launches++;
     }
     CK(ctx, cudaEventRecord(s.ev_res, st));  // kernel(s) done => sizes + digests are in host memory
     return SKY_OK;
@@ -1353,7 +1397,7 @@ int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64
                        void *d_dst, const uint64_t *dst_off, const uint64_t *dst_cap, uint32_t flags, void *stream,
                        uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
     if (!ctx || n == 0 || !src_off || !src_len || !dst_off || !dst_cap || !d_dst) return SKY_E_INVALID;
-    if (flags & (SKY_F_E2EE | SKY_F_VERIFY)) return SKY_E_INVALID;  // host-path features (sky_submit; sky_verify_device checks)
+    if (flags & (SKY_F_E2EE | SKY_F_VERIFY | SKY_F_PASSTHROUGH)) return SKY_E_INVALID;  // host-path features (sky_submit; sky_verify_device checks)
     if (!frame_flags_valid(flags)) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
     if ((reinterpret_cast<uintptr_t>(d_src) & 15) || (reinterpret_cast<uintptr_t>(d_dst) & 15)) return SKY_E_INVALID;
@@ -1419,7 +1463,10 @@ int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t 
     return SKY_OK;
 }
 
-int sky_wait_verify(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, float *kernel_ms) {
+// The waits: sky_wait_ex (compressed != NULL) completes any ticket; sky_wait and sky_wait_verify (compressed == NULL) refuse
+// a SKY_F_PASSTHROUGH ticket, whose payloads are not all frames.
+static int wait_ticket(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, uint8_t *compressed,
+                       float *kernel_ms) {
     if (!ctx) return SKY_E_INVALID;
     Slot *sp = nullptr;
     for (Slot &s : ctx->slots)
@@ -1427,6 +1474,7 @@ int sky_wait_verify(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *m
     if (!sp) return SKY_E_TICKET;
     Slot &s = *sp;
     if (verify && !(s.ticket.flags & SKY_F_VERIFY)) return SKY_E_INVALID;  // (the ticket stays valid)
+    if (!compressed && (s.ticket.flags & SKY_F_PASSTHROUGH)) return SKY_E_INVALID;  // (likewise)
     CK(ctx, cudaSetDevice(ctx->device));
     { int prc = progress(ctx); if (prc != SKY_OK) return prc; }
     if (!s.ticket.d2h_issued) {
@@ -1439,20 +1487,36 @@ int sky_wait_verify(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *m
     if (out_len) memcpy(out_len, s.meta.outlen.h, s.ticket.n * sizeof(uint64_t));
     if (md5) memcpy(md5, s.meta.md5.h, (size_t)s.ticket.n * 16);
     if (verify) memcpy(verify, s.verify.status.h, s.ticket.n * sizeof(int32_t));
+    if (compressed) {
+        if (s.ticket.flags & SKY_F_PASSTHROUGH)
+            for (uint32_t i = 0; i < s.ticket.n; i++) compressed[i] = s.meta.pass.h[i] ? 0 : 1;
+        else
+            memset(compressed, (s.ticket.flags & SKY_F_LZ4) ? 1 : 0, s.ticket.n);
+    }
     if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, s.ev_k0, s.ev_k1));
     s.ticket.busy = false;
     return SKY_OK;
 }
 
+int sky_wait_verify(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, float *kernel_ms) {
+    return wait_ticket(ctx, ticket, out_len, md5, verify, nullptr, kernel_ms);
+}
+
 int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
-    return sky_wait_verify(ctx, ticket, out_len, md5, nullptr, kernel_ms);
+    return wait_ticket(ctx, ticket, out_len, md5, nullptr, nullptr, kernel_ms);
+}
+
+int sky_wait_ex(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, uint8_t *compressed, float *kernel_ms) {
+    if (!compressed) return SKY_E_INVALID;
+    return wait_ticket(ctx, ticket, out_len, md5, verify, compressed, kernel_ms);
 }
 
 int sky_verify_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64_t *src_off, const uint64_t *src_len, void *d_frames,
                       const uint64_t *frame_off, uint64_t *frame_len, const uint64_t *frame_cap, const uint32_t *content_xxh,
                       uint32_t flags, void *stream, int32_t *status, float *kernel_ms) {
     if (!ctx || n == 0 || !src_off || !src_len || !d_frames || !frame_off || !frame_len) return SKY_E_INVALID;
-    if ((flags & SKY_F_E2EE) || !frame_flags_valid(flags) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) == SKY_F_MD5) return SKY_E_INVALID;
+    if ((flags & (SKY_F_E2EE | SKY_F_PASSTHROUGH)) || !frame_flags_valid(flags) || (flags & (SKY_F_LZ4 | SKY_F_MD5)) == SKY_F_MD5)
+        return SKY_E_INVALID;
     if (((flags & SKY_F_CHECKSUM) != 0) != (content_xxh != nullptr)) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
     if (reinterpret_cast<uintptr_t>(d_src) & 15) return SKY_E_INVALID;

@@ -37,6 +37,8 @@ def _drain_status(store: ChunkStore, acc: Dict):
                 acc["raw"] += rec.get("uncompressed_size_bytes", 0)
                 if "frame_verify_status" in rec:
                     acc["verify"][rec["chunk_id"]] = rec["frame_verify_status"]
+                if rec.get("passed_through"):
+                    acc["passed_through"].add(rec["chunk_id"])
     except queue.Empty:
         pass
 
@@ -64,16 +66,18 @@ def run_stream(
     verify_frames: bool = False,
     block_linked: bool = False,
     optimal_parse: bool = False,
+    skip_incompressible: bool = False,
 ) -> Dict:
     """Stream ``n_requests`` chunk requests (recycling ``pool_files`` by hard link) through the operator.
 
     The first ``warmup_requests`` completions are not timed (worker start-up: CUDA context, pinned staging).
-    ``high_ratio``, ``content_checksum``, ``compression_level``, ``block_checksum``, ``verify_frames``, ``block_linked`` and
-    ``optimal_parse`` are handed to the operator (GatewayCompressHash's high-ratio frames, frames with LZ4's content
-    checksum, the high-ratio level, frames with LZ4's block checksums, the GPU's check of every frame, linked blocks, the
-    optimal parse) when set.
+    ``high_ratio``, ``content_checksum``, ``compression_level``, ``block_checksum``, ``verify_frames``, ``block_linked``,
+    ``optimal_parse`` and ``skip_incompressible`` are handed to the operator (GatewayCompressHash's high-ratio frames, frames
+    with LZ4's content checksum, the high-ratio level, frames with LZ4's block checksums, the GPU's check of every frame,
+    linked blocks, the optimal parse, incompressible chunks sent as themselves) when set.
     Returns {"wall_s", "bytes", "records": [{chunk_id, pool_index, md5, raw_len, frame_path}], "status": {...},
-    "frame_verify": {chunk_id: status of every chunk whose frame failed the check}}.
+    "frame_verify": {chunk_id: status of every chunk whose frame failed the check},
+    "passed_through": [chunk_id of every chunk sent as itself]}.
     """
     chunk_dir = Path(chunk_dir)
     store = ChunkStore(chunk_dir)
@@ -90,10 +94,11 @@ def run_stream(
         **({"verify_frames": True} if verify_frames else {}),
         **({"block_linked": True} if block_linked else {}),
         **({"optimal_parse": True} if optimal_parse else {}),
+        **({"skip_incompressible": True} if skip_incompressible else {}),
     )
     op.start_workers()
     records: List[Dict] = []
-    status_acc = {"states": {}, "comp": 0, "raw": 0, "verify": {}}
+    status_acc = {"states": {}, "comp": 0, "raw": 0, "verify": {}, "passed_through": set()}
     pool_of: Dict[str, int] = {}
     sent = done = 0
     total_bytes = 0
@@ -164,7 +169,7 @@ def run_stream(
     store.chunk_status_queue.cancel_join_thread()
     status, comp, raw = status_acc["states"], status_acc["comp"], status_acc["raw"]
     return {"wall_s": wall, "bytes": total_bytes, "records": records, "status": status, "compressed_bytes": comp, "uncompressed_bytes": raw,
-            "frame_verify": status_acc["verify"]}
+            "frame_verify": status_acc["verify"], "passed_through": sorted(status_acc["passed_through"])}
 
 
 def main():

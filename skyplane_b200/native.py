@@ -19,6 +19,8 @@ F_LZ4, F_MD5, F_E2EE, F_HC, F_CHECKSUM, F_BLOCK_CHECKSUM = 1, 2, 16, 32, 64, 128
 F_VERIFY = 1 << 12  # every frame is checked against its chunk on the GPU; one that fails is sent as its stored-block frame
 F_LINKED = 1 << 13  # with F_HC only: linked blocks (python-lz4's block_linked), matches may reach into the previous 64 KiB
 F_OPTIMAL = 1 << 14  # with F_HC only: the optimal parse (sequences chosen by their cost in bytes) over the same match search
+# sky_submit only, with F_LZ4: a chunk whose frame is not smaller than the chunk is sent as itself (wait_ex says which)
+F_PASSTHROUGH = 1 << 15
 CHECKSUM_BYTES = 4  # F_CHECKSUM: the content checksum (u32le XXH32) behind the EndMark; F_BLOCK_CHECKSUM: as many per block
 BLOCK_BYTES = 65536
 # SKY_F_HC_LEVEL(l): the high-ratio level l (3..9: 2**(l - 1) chain candidates per position) in bits 8..11 of the flags;
@@ -38,7 +40,7 @@ D_NAMES = {0: "ok", -1: "bad frame header", -2: "corrupt block", -3: "size misma
 ABI_SYMBOLS = (
     "sky_strerror", "sky_last_error", "sky_abi_version", "sky_device_count", "sky_device_pci_bus_id", "sky_kernel_config", "sky_frame_bound",
     "sky_ctx_create", "sky_ctx_destroy", "sky_pinned_alloc", "sky_pinned_free",
-    "sky_submit", "sky_wait", "sky_wait_verify", "sky_set_e2ee_key", "sky_box_bound", "sky_process_device", "sky_verify_device",
+    "sky_submit", "sky_wait", "sky_wait_verify", "sky_wait_ex", "sky_set_e2ee_key", "sky_box_bound", "sky_process_device", "sky_verify_device",
     "sky_decode_device", "sky_decode",
     "sky_device_alloc", "sky_device_free", "sky_memcpy_h2d", "sky_memcpy_d2h", "sky_launch_count",
 )
@@ -113,6 +115,8 @@ def lib() -> ctypes.CDLL:
     L.sky_wait.restype = i32
     L.sky_wait_verify.argtypes = [vp, u64, p_u64, vp, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_float)]
     L.sky_wait_verify.restype = i32
+    L.sky_wait_ex.argtypes = [vp, u64, p_u64, vp, ctypes.POINTER(ctypes.c_int32), vp, ctypes.POINTER(ctypes.c_float)]
+    L.sky_wait_ex.restype = i32
     L.sky_process_device.argtypes = [vp, u32, vp, p_u64, p_u64, vp, p_u64, p_u64, u32, vp, p_u64, vp, ctypes.POINTER(ctypes.c_float)]
     L.sky_process_device.restype = i32
     p_i32 = ctypes.POINTER(ctypes.c_int32)
@@ -199,9 +203,21 @@ def frame_need(n: int, checksum: bool = False, block_checksum: bool = False) -> 
     return frame_bound(n) + (CHECKSUM_BYTES if checksum else 0) + (CHECKSUM_BYTES * blocks if block_checksum else 0)
 
 
+def check_passthrough(compress: bool = True, checksum: bool = False, block_checksum: bool = False):
+    """F_PASSTHROUGH's rules, where the sender's options are chosen (so a bad combination fails when a stage call or an
+    operator is set up, not in a worker): it chooses per chunk between the frame and the chunk, so it needs compression, and
+    a chunk sent as itself cannot carry the LZ4 content or block checksums asked for.  ValueError otherwise."""
+    if not compress:
+        raise ValueError("pass-through chooses between a chunk's LZ4 frame and the chunk: it needs compression")
+    if checksum:
+        raise ValueError("pass-through does not combine with the content checksum: a chunk sent as itself has no LZ4 frame to carry it")
+    if block_checksum:
+        raise ValueError("pass-through does not combine with block checksums: a chunk sent as itself has no LZ4 frame to carry them")
+
+
 _DECODE_ONLY_SUBMIT = ((F_HC, "F_HC"), (HC_LEVEL_MASK, "a high-ratio level"), (F_CHECKSUM, "F_CHECKSUM"),
                        (F_BLOCK_CHECKSUM, "F_BLOCK_CHECKSUM"), (F_VERIFY, "F_VERIFY"), (F_LINKED, "F_LINKED"),
-                       (F_OPTIMAL, "F_OPTIMAL"))
+                       (F_OPTIMAL, "F_OPTIMAL"), (F_PASSTHROUGH, "F_PASSTHROUGH"))
 
 
 def check_decode_flags(flags: int) -> int:
@@ -323,7 +339,10 @@ class Context:
 
     def submit(self, src_addrs: Sequence[int], src_lens: Sequence[int], dst_addrs: Optional[Sequence[int]], dst_caps: Optional[Sequence[int]],
                flags: int = 0, nonces: Optional[bytes] = None) -> int:
-        """flags = F_MD5: digests only (dst may be None). | F_E2EE: dst receives sealed boxes; nonces = 24 bytes per chunk."""
+        """flags = F_MD5: digests only (dst may be None). | F_E2EE: dst receives sealed boxes; nonces = 24 bytes per chunk.
+        | F_PASSTHROUGH: chunks whose frame does not shrink them are sent as themselves; complete the ticket with wait_ex."""
+        if flags & F_PASSTHROUGH:
+            check_passthrough((flags & (F_LZ4 | F_MD5)) != F_MD5, bool(flags & F_CHECKSUM), bool(flags & F_BLOCK_CHECKSUM))
         n = len(src_addrs)
         A = ctypes.c_void_p * n
         U = ctypes.c_uint64 * n
@@ -332,12 +351,12 @@ class Context:
             raise ValueError("need 24 nonce bytes per chunk")
         t = ctypes.c_uint64(0)
         self._check(lib().sky_submit(self._h, n, args[0], args[1], args[2], args[3], flags, nonces, ctypes.byref(t)))
-        self._inflight[t.value] = (n, args)  # keep the pointer arrays alive until wait()
+        self._inflight[t.value] = (n, args, flags)  # keep the pointer arrays alive until wait()
         return t.value
 
     def wait(self, ticket: int):
         """-> (out_lens: list[int], digests: list[bytes], kernel_ms: float)"""
-        n, _keep = self._inflight.pop(ticket)
+        n, _keep, _flags = self._inflight.pop(ticket)
         out = (ctypes.c_uint64 * n)()
         md5 = (ctypes.c_ubyte * (16 * n))()
         ms = ctypes.c_float(0)
@@ -348,7 +367,7 @@ class Context:
     def wait_verify(self, ticket: int):
         """wait() for a ticket submitted with F_VERIFY -> (out_lens, digests, verify, kernel_ms); verify[i] is 0 or the D_*
         code of chunk i's frame as the compressor made it (its payload is then the stored-block frame)."""
-        n, _keep = self._inflight[ticket]
+        n, _keep, _flags = self._inflight[ticket]
         out = (ctypes.c_uint64 * n)()
         md5 = (ctypes.c_ubyte * (16 * n))()
         ver = (ctypes.c_int32 * n)()
@@ -357,6 +376,23 @@ class Context:
         del self._inflight[ticket]
         raw = bytes(md5)
         return list(out), [raw[16 * i : 16 * i + 16] for i in range(n)], list(ver), ms.value
+
+    def wait_ex(self, ticket: int):
+        """Completes any ticket, and the only wait for one submitted with F_PASSTHROUGH -> (out_lens, digests, verify,
+        compressed, kernel_ms).  compressed[i]: True when chunk i's payload is its frame (or the box of its frame), False when
+        it is the chunk (out_len 0 without F_E2EE: the caller holds the bytes) or the box of the chunk.  verify is None unless
+        the ticket has F_VERIFY."""
+        n, _keep, flags = self._inflight[ticket]
+        out = (ctypes.c_uint64 * n)()
+        md5 = (ctypes.c_ubyte * (16 * n))()
+        comp = (ctypes.c_uint8 * n)()
+        ms = ctypes.c_float(0)
+        has_verify = bool(flags & F_VERIFY)
+        ver = (ctypes.c_int32 * n)() if has_verify else None
+        self._check(lib().sky_wait_ex(self._h, ticket, out, md5, ver, comp, ctypes.byref(ms)))
+        del self._inflight[ticket]
+        raw = bytes(md5)
+        return list(out), [raw[16 * i : 16 * i + 16] for i in range(n)], list(ver) if has_verify else None, [bool(c) for c in comp], ms.value
 
     # ------------------------------------------------------------------ device-resident path
     def process_device(self, d_src: int, src_off: Sequence[int], src_len: Sequence[int], d_dst: int, dst_off: Sequence[int],

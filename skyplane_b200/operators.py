@@ -143,6 +143,7 @@ class GatewayCompressHash(GatewayOperator):
         verify_frames: bool = False,
         block_linked: bool = False,
         optimal_parse: bool = False,
+        skip_incompressible: bool = False,
     ):
         """use_compression / e2ee_key_bytes: GatewaySender's arguments of the same name (gateway_operator.py:154-168):
         ``use_compression=False`` digests the chunk and lets it pass through uncompressed (``is_compressed=False``);
@@ -166,6 +167,12 @@ class GatewayCompressHash(GatewayOperator):
         optimal_parse: the high-ratio frames with the optimal parse (``ChunkStage.launch(optimal=True)``): the same match
         search, sequences chosen by their cost in bytes, so fewer bytes at the same level for more GPU time.  The frame
         format and receiver stay the same.  Off by default.  Needs ``high_ratio`` or a ``compression_level`` of 3..9.
+        skip_incompressible: a chunk whose LZ4 frame is not smaller than the chunk is sent as itself
+        (``ChunkStage.launch(passthrough=True)``, ``is_compressed=False`` for that chunk only): without a key no payload file
+        is written for it (``<chunk_id>.chunk`` is the payload), with a key its SecretBox goes to ``<chunk_id>.chunk.box``;
+        its ``complete`` record carries ``"passed_through": true``.  Every other chunk's payload is what it is without this
+        option.  Needs ``use_compression``; refused with ``content_checksum`` or ``block_checksum``, which a chunk sent as
+        itself cannot carry.
         sink: ``callable(worker_id) -> socket``, called once in each worker.  With a sink the worker sends every payload
         straight from the pinned staging slot (``wire.send_results``: WireProtocolHeader + payload, no intermediate bytes
         object, no frame file) -- the tail of ``GatewaySender.process`` (gateway_operator.py:367-402)."""
@@ -192,6 +199,9 @@ class GatewayCompressHash(GatewayOperator):
         if optimal_parse and not hc_bits:
             raise ValueError("optimal_parse is a parse of the high-ratio compressor: it needs high_ratio or a compression_level of 3..9")
         self.optimal_parse = bool(optimal_parse)
+        if skip_incompressible:
+            native.check_passthrough(self.use_compression, self.content_checksum, self.block_checksum)
+        self.skip_incompressible = bool(skip_incompressible)
         self.compression_level = compression_level
         self.e2ee_key_bytes = e2ee_key_bytes
         self.sink = sink
@@ -348,6 +358,8 @@ class GatewayCompressHash(GatewayOperator):
             opts["linked"] = True
         if self.optimal_parse:
             opts["optimal"] = True
+        if self.skip_incompressible:
+            opts["passthrough"] = True
         stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None, **opts)
         return True
 
@@ -369,6 +381,8 @@ class GatewayCompressHash(GatewayOperator):
         for r, res in zip(reqs, results):
             r.chunk.md5_hash = res.md5
             r._stage_meta = {"compressed_size_bytes": res.comp_len, "uncompressed_size_bytes": res.raw_len}
+            if self.skip_incompressible and not res.is_compressed:
+                r._stage_meta["passed_through"] = True
             if res.verify_status:
                 from skyplane_b200 import native
 
@@ -385,7 +399,8 @@ class GatewayCompressHash(GatewayOperator):
         elif self.keep_frames_on_disk:
             for r, res in zip(reqs, results):
                 if res.is_compressed or res.is_encrypted:  # (a plain pass-through chunk is already on disk as <id>.chunk)
-                    path = self.chunk_store.get_compressed_file_path(r.chunk.chunk_id)
+                    sealed_raw = self.skip_incompressible and not res.is_compressed  # a chunk of a compressed transfer sent as itself
+                    path = (self.chunk_store.get_box_file_path if sealed_raw else self.chunk_store.get_compressed_file_path)(r.chunk.chunk_id)
                     tmp = path.with_name(path.name + ".part")
                     with open(tmp, "wb") as f:
                         f.write(res.frame)
@@ -501,13 +516,23 @@ class GatewayDecompressVerify(GatewayOperator):
     ``<chunk_id>.chunk.lz4`` is the SecretBox of the chunk: it is opened and digested on the GPU and written as
     ``<chunk_id>.chunk``.  Without a key the payload is the chunk, which the receiver has already written as
     ``<chunk_id>.chunk`` (gateway_receiver.py:204-224): that file is read, digested on the GPU and compared with
-    ``chunk.md5_hash``, and is not rewritten; while its size is not ``chunk_length_bytes`` it counts as still arriving."""
+    ``chunk.md5_hash``, and is not rewritten; while its size is not ``chunk_length_bytes`` it counts as still arriving.
+
+    ``skip_incompressible=True`` is the receiving side of ``GatewayCompressHash(skip_incompressible=True)``, whose stream
+    mixes frames and chunks sent as themselves.  Each request is routed by the file its payload arrived as:
+    ``<chunk_id>.chunk.lz4`` is decoded (opened first with a key), ``<chunk_id>.chunk.box`` (with a key) is opened as the
+    sealed chunk, and otherwise (without a key) ``<chunk_id>.chunk`` is the chunk itself, digested where it lies.  Each
+    route's requests go through one decode call and keep that route's rules for payloads still arriving.  Needs
+    ``use_compression``."""
 
     def __init__(self, *args, max_batch_chunks: int = 64, max_batch_bytes: int = 512 << 20, n_gpus: Optional[int] = None,
                  remove_frames: bool = True, e2ee_key_bytes: Optional[bytes] = None, stale_retries: int = 50,
-                 use_compression: bool = True, **kwargs):
+                 use_compression: bool = True, skip_incompressible: bool = False, **kwargs):
         super().__init__(*args, **kwargs)
         self.use_compression = True if use_compression is None else bool(use_compression)
+        if skip_incompressible and not self.use_compression:
+            raise ValueError("skip_incompressible receives a compressed transfer's mixed stream: it needs use_compression")
+        self.skip_incompressible = bool(skip_incompressible)
         self.max_batch_chunks = max_batch_chunks
         self.max_batch_bytes = max_batch_bytes
         self.n_gpus = n_gpus
@@ -546,33 +571,50 @@ class GatewayDecompressVerify(GatewayOperator):
         self._seen[chunk_id] = (size, tries)
         return tries <= self.stale_retries
 
+    def _routes(self):
+        """-> [(payload path of a chunk id, compressed, encrypted)]: where a request's payload is looked for, in order, and what
+        it is when found there."""
+        cs = self.chunk_store
+        encrypted = self.e2ee_key_bytes is not None
+        if not self.skip_incompressible:
+            in_place = not self.use_compression and not encrypted  # the payload is the chunk: <chunk_id>.chunk, digested where it lies
+            return [(cs.get_chunk_file_path if in_place else cs.get_compressed_file_path, self.use_compression, encrypted)]
+        raw = (cs.get_box_file_path, False, True) if encrypted else (cs.get_chunk_file_path, False, False)
+        return [(cs.get_compressed_file_path, True, encrypted), raw]
+
     def process_batch(self, reqs: List[ChunkRequest]) -> List[bool]:
         """One bool per request: False = payload not there / not complete yet (re-queue)."""
-        from skyplane_b200 import native
-
         ok = [False] * len(reqs)
-        ready, frames = [], []
-        total = 0
-        encrypted = self.e2ee_key_bytes is not None
-        in_place = not self.use_compression and not encrypted  # the payload is the chunk: <chunk_id>.chunk, digested where it lies
-        payload_path = self.chunk_store.get_chunk_file_path if in_place else self.chunk_store.get_compressed_file_path
+        groups = {}  # route -> [(request index, payload)], one decode call each
+        routes = self._routes()
+        total, ready = 0, False
         for i, r in enumerate(reqs):
-            fpath = payload_path(r.chunk.chunk_id)
-            try:
-                frame = fpath.read_bytes()
-            except FileNotFoundError:
+            for route in routes:
+                try:
+                    frame = route[0](r.chunk.chunk_id).read_bytes()
+                    break
+                except FileNotFoundError:
+                    continue
+            else:
                 continue  # payload not received yet: retry
             if total + len(frame) + r.chunk.chunk_length_bytes > self.max_batch_bytes and ready:
                 continue  # next batch
             total += len(frame) + r.chunk.chunk_length_bytes
-            ready.append(i)
-            frames.append(frame)
-        if not ready:
-            return ok
-        raw = {} if self.use_compression else {"compressed": False}
-        out = self._get_stage().decode(frames, [reqs[i].chunk.chunk_length_bytes for i in ready], encrypted=encrypted, **raw)
+            ready = True
+            groups.setdefault(route, []).append((i, frame))
+        for route, items in groups.items():
+            self._receive(reqs, items, *route, ok)
+        return ok
+
+    def _receive(self, reqs: List[ChunkRequest], items, payload_path, compressed: bool, encrypted: bool, ok: List[bool]):
+        """Decode / open / digest one route's payloads and write the chunks; ok[i] = True for every request done."""
+        from skyplane_b200 import native
+
+        in_place = not compressed and not encrypted
+        raw = {} if compressed else {"compressed": False}
+        out = self._get_stage().decode([f for _, f in items], [reqs[i].chunk.chunk_length_bytes for i, _ in items], encrypted=encrypted, **raw)
         arriving = (native.D_TRUNCATED, native.D_BAD_HEADER, native.D_AUTH) + ((native.D_SIZE,) if in_place else ())
-        for i, frame, (data, digest, status) in zip(ready, frames, out):
+        for (i, frame), (data, digest, status) in zip(items, out):
             chunk = reqs[i].chunk
             if status in arriving and self._still_arriving(chunk.chunk_id, len(frame)):
                 continue  # a writer may still be appending (a short box fails authentication, a short frame is truncated,
@@ -595,9 +637,8 @@ class GatewayDecompressVerify(GatewayOperator):
             chunk.md5_hash = digest  # lets the upload step send Content-MD5 (gateway_operator.py:640)
             self._seen.pop(chunk.chunk_id, None)
             if self.remove_frames and not in_place:
-                self.chunk_store.get_compressed_file_path(chunk.chunk_id).unlink(missing_ok=True)
+                payload_path(chunk.chunk_id).unlink(missing_ok=True)
             ok[i] = True
-        return ok
 
     def worker_loop(self, worker_id: int, *args):
         """Batch-draining loop with the reference's logging / error conventions (gateway_operator.py:79-115)."""

@@ -38,6 +38,7 @@ def _compress_hash(op: Dict, kw: Dict) -> GatewayOperator:
         verify_frames=op.get("verify_frames", False),
         block_linked=op.get("block_linked", False),
         optimal_parse=op.get("optimal_parse", False),
+        skip_incompressible=op.get("skip_incompressible", False),
         max_batch_chunks=op.get("max_batch_chunks", 64),
         max_batch_bytes=op.get("max_batch_bytes", 512 << 20),
         n_gpus=op.get("num_gpus"),
@@ -46,8 +47,9 @@ def _compress_hash(op: Dict, kw: Dict) -> GatewayOperator:
 
 def _decompress_verify(op: Dict, kw: Dict) -> GatewayOperator:
     # "compress" as on compress_hash and the reference's send / receive nodes: false when the sender's is false
+    # "skip_incompressible" as on compress_hash: the stream mixes frames and chunks sent as themselves
     return GatewayDecompressVerify(**kw, n_processes=op.get("num_gpus", 1), n_gpus=op.get("num_gpus"),
-                                   use_compression=op.get("compress", True))
+                                   use_compression=op.get("compress", True), skip_incompressible=op.get("skip_incompressible", False))
 
 
 def _receive(op: Dict, kw: Dict) -> GatewayOperator:

@@ -24,11 +24,12 @@ class StageResult:
     """What the sender needs for one chunk (gateway_operator.py:367-372)."""
 
     frame: memoryview  # wire payload (view into the slot's pinned memory; valid until the slot is reused): the LZ4 frame,
-    #                    or the chunk itself when compression is off, sealed in a SecretBox when E2EE is on
+    #                    or the chunk itself when compression is off or the chunk passed through, sealed in a SecretBox when
+    #                    E2EE is on
     md5: bytes  # 16 raw bytes == hashlib.md5(chunk).digest()
     raw_len: int  # WireProtocolHeader.raw_data_len
     comp_len: int  # WireProtocolHeader.data_len (length of `frame`)
-    is_compressed: bool = True  # WireProtocolHeader.is_compressed
+    is_compressed: bool = True  # WireProtocolHeader.is_compressed (per chunk: launch(passthrough=True) sends some chunks as themselves)
     is_encrypted: bool = False
     verify_status: int = 0  # launch(verify=True): 0, or the native.D_* code of the frame as compressed (`frame` is then the
     #                         chunk's stored-block frame)
@@ -174,7 +175,7 @@ class ChunkStage:
 
     def launch(self, slot: _Slot, compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None, hc: bool = False,
                checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False, verify: bool = False,
-               linked: bool = False, optimal: bool = False) -> _Slot:
+               linked: bool = False, optimal: bool = False, passthrough: bool = False) -> _Slot:
         """compress=False is the reference's `compress: false` (digest only, the chunk passes through);
         encrypt=True seals every payload with the stage's key (nonces: 24 bytes per chunk, default os.urandom);
         hc=True makes the frames with the high-ratio parse (F_HC): same frame format, fewer bytes, more GPU time;
@@ -191,7 +192,11 @@ class ChunkStage:
         order.  It needs the high-ratio mode (hc=True or a level 3..9);
         optimal=True makes the high-ratio frames with the optimal parse (F_OPTIMAL): the same match search, sequences chosen
         by their cost in bytes, about 1.3 % fewer bytes at level 5 for 4 % more GPU time.  It needs the high-ratio mode
-        too, and combines with linked and every level."""
+        too, and combines with linked and every level;
+        passthrough=True sends every chunk whose frame is not smaller than the chunk as the chunk itself (F_PASSTHROUGH):
+        its StageResult has is_compressed=False and, without encrypt, `frame` is the chunk in the input slot, which is not
+        copied back from the GPU; with encrypt it is the box of the chunk.  The other chunks' frames are unchanged.  It needs
+        compress=True and refuses checksum and block_checksum, which a chunk sent as itself cannot carry."""
         if not slot.lens:
             raise ValueError("empty batch")
         if hc and not compress:
@@ -202,6 +207,8 @@ class ChunkStage:
             raise ValueError("block_checksum=True is carried by the LZ4 frame: it needs compress=True")
         if verify and not compress:
             raise ValueError("verify=True checks the LZ4 frames: it needs compress=True")
+        if passthrough:
+            native.check_passthrough(compress, checksum, block_checksum)
         hc_bits = native.hc_flags(level, hc, compress)
         _check_hc_modes(linked, optimal, hc_bits)
         if hc_bits and not native.kernel_config()["hc_depth"]:
@@ -214,7 +221,8 @@ class ChunkStage:
         src = [base_in + o for o in slot.in_off]
         flags = (native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0) | hc_bits
                  | (native.F_CHECKSUM if checksum else 0) | (native.F_BLOCK_CHECKSUM if block_checksum else 0)
-                 | (native.F_VERIFY if verify else 0) | (native.F_LINKED if linked else 0) | (native.F_OPTIMAL if optimal else 0))
+                 | (native.F_VERIFY if verify else 0) | (native.F_LINKED if linked else 0) | (native.F_OPTIMAL if optimal else 0)
+                 | (native.F_PASSTHROUGH if passthrough else 0))
         if encrypt and nonces is None:
             nonces = os.urandom(24 * len(slot.lens))  # what nacl.utils.random(24) draws per message
         if compress or encrypt:
@@ -228,16 +236,21 @@ class ChunkStage:
         return slot
 
     def collect(self, slot: _Slot) -> List[StageResult]:
-        if slot.flags & native.F_VERIFY:
+        comp, enc = bool(slot.flags & native.F_LZ4), bool(slot.flags & native.F_E2EE)
+        if slot.flags & native.F_PASSTHROUGH:
+            out_lens, digests, verify, compressed, self.last_kernel_ms = self.ctx.wait_ex(slot.ticket)
+            verify = verify or [0] * len(slot.lens)
+        elif slot.flags & native.F_VERIFY:
             out_lens, digests, verify, self.last_kernel_ms = self.ctx.wait_verify(slot.ticket)
+            compressed = [comp] * len(slot.lens)
         else:
             out_lens, digests, self.last_kernel_ms = self.ctx.wait(slot.ticket)
             verify = [0] * len(slot.lens)
-        comp, enc = bool(slot.flags & native.F_LZ4), bool(slot.flags & native.F_E2EE)
+            compressed = [comp] * len(slot.lens)
         res = []
-        for io, o, cl, dg, n, v in zip(slot.in_off, slot.out_off, out_lens, digests, slot.lens, verify):
-            payload = slot.out.view[o : o + cl] if (comp or enc) else slot.inp.view[io : io + n]
-            res.append(StageResult(frame=payload, md5=dg, raw_len=n, comp_len=len(payload), is_compressed=comp, is_encrypted=enc,
+        for io, o, cl, dg, n, v, c in zip(slot.in_off, slot.out_off, out_lens, digests, slot.lens, verify, compressed):
+            payload = slot.out.view[o : o + cl] if (c or enc) else slot.inp.view[io : io + n]
+            res.append(StageResult(frame=payload, md5=dg, raw_len=n, comp_len=len(payload), is_compressed=c, is_encrypted=enc,
                                    verify_status=v))
         slot.ticket = None
         self._free.append(slot)
@@ -246,9 +259,11 @@ class ChunkStage:
     # ------------------------------------------------------------------ sync convenience
     def process(self, chunks: Sequence[BytesLike], compress: bool = True, encrypt: bool = False, nonces: Optional[bytes] = None,
                 hc: bool = False, checksum: bool = False, level: Optional[int] = None, block_checksum: bool = False,
-                verify: bool = False, linked: bool = False, optimal: bool = False) -> List[StageResult]:
+                verify: bool = False, linked: bool = False, optimal: bool = False, passthrough: bool = False) -> List[StageResult]:
         """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes (hc, checksum,
-        level, block_checksum, verify, linked, optimal: see launch)."""
+        level, block_checksum, verify, linked, optimal, passthrough: see launch)."""
+        if passthrough:
+            native.check_passthrough(compress, checksum, block_checksum)
         _check_hc_modes(linked, optimal, native.hc_flags(level, hc, compress))  # (bad arguments fail before the first batch)
         if block_checksum and not compress:
             raise ValueError("block_checksum=True is carried by the LZ4 frame: it needs compress=True")
@@ -266,7 +281,7 @@ class ChunkStage:
                 self.release(slot)
                 raise native.SkyChunkError(native.SKY_E_CAPACITY, f"chunk of {memoryview(chunks[i]).nbytes} bytes exceeds max_batch_bytes")
             self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum, level, block_checksum,
-                        verify, linked, optimal)
+                        verify, linked, optimal, passthrough)
             for r in self.collect(slot):
                 out.append(StageResult(frame=memoryview(bytes(r.frame)), md5=r.md5, raw_len=r.raw_len, comp_len=r.comp_len,
                                        is_compressed=r.is_compressed, is_encrypted=r.is_encrypted, verify_status=r.verify_status))
