@@ -19,11 +19,11 @@
 //   place  : the OFF chain gives the block's frame offset (place_block), and all warps copy it there.
 // Claim, load, placement and write-out are frame.cuh's, shared with sky_fused_kernel.
 //
-// Optimal parse (SKY_F_OPTIMAL, sky_hc_opt{,_bc,_linked,_linked_bc}_kernel): between search and emission every warp
+// Optimal parse (SKY_F_OPTIMAL, sky_hc_kernel's kOpt): between search and emission every warp
 // parses its own 2 KiB segment of the block by the bytes the sequences cost (opt_segment, the twin's
 // hc_compress_block_opt), and warp 0 then emits the matches the segments chose instead of the lazy parse's.
 //
-// Linked blocks (SKY_F_LINKED, sky_hc_linked{,_bc}_kernel): block j >= 1 of a chunk also sees the chunk's 64 KiB before it
+// Linked blocks (SKY_F_LINKED, sky_hc_kernel's kLinked): block j >= 1 of a chunk also sees the chunk's 64 KiB before it
 // (the twin's hc_compress_block_linked).  Shared memory has no room for that window, so it stays where it is:
 //   window bytes : read from the chunk in global memory (d.src - 65536, L2-resident) by load32x / load8x, which read shared
 //                  memory for a position in the block and global memory for one before it;
@@ -158,7 +158,7 @@ __device__ __forceinline__ void opt_segment(uint32_t in_s, const uint8_t *src, u
 // checksum (block_checksum), hashed from the frame by warp 1 during the next block's chain step, which only warp 0 works
 // on (or before the CTA exits).  kLinked (SKY_F_LINKED): blocks after a chunk's first match into its previous 64 KiB.
 // kOpt (SKY_F_OPTIMAL): every warp parses its segment optimally (opt_segment) before warp 0 emits the chosen matches.
-template <uint32_t kHcDepth, bool kBlkChk, bool kLinked = false, bool kOpt = false>
+template <uint32_t kHcDepth, bool kBlkChk, bool kLinked, bool kOpt>
 __device__ __forceinline__ void hc_body(const Params &p) {
     extern __shared__ __align__(128) uint8_t smem[];
     const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -378,24 +378,9 @@ __device__ __forceinline__ void hc_body(const Params &p) {
     }
 }
 
-template <uint32_t kHcDepth>
-__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) { hc_body<kHcDepth, false>(p); }
-// SKY_F_BLOCK_CHECKSUM: the same kernel with block checksums.
-template <uint32_t kHcDepth>
-__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_bc_kernel(const Params p) { hc_body<kHcDepth, true>(p); }
-// SKY_F_LINKED: both with linked blocks (kHcLinkedSmemBytes of shared memory, kHcLinkedScratchBytes of scratch per CTA).
-template <uint32_t kHcDepth>
-__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_linked_kernel(const Params p) { hc_body<kHcDepth, false, true>(p); }
-template <uint32_t kHcDepth>
-__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_linked_bc_kernel(const Params p) { hc_body<kHcDepth, true, true>(p); }
-// SKY_F_OPTIMAL: the four with the optimal parse (same shared memory and scratch as their lazy counterparts).
-template <uint32_t kHcDepth>
-__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_opt_kernel(const Params p) { hc_body<kHcDepth, false, false, true>(p); }
-template <uint32_t kHcDepth>
-__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_opt_bc_kernel(const Params p) { hc_body<kHcDepth, true, false, true>(p); }
-template <uint32_t kHcDepth>
-__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_opt_linked_kernel(const Params p) { hc_body<kHcDepth, false, true, true>(p); }
-template <uint32_t kHcDepth>
-__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_opt_linked_bc_kernel(const Params p) { hc_body<kHcDepth, true, true, true>(p); }
+// Linked kernels take kHcLinkedSmemBytes of shared memory and kHcLinkedScratchBytes of scratch per CTA, the others
+// kHcSmemBytes and kHcScratchBytes; the optimal parse needs no more than the lazy one.
+template <uint32_t kHcDepth, bool kBlkChk, bool kLinked, bool kOpt>
+__global__ void __launch_bounds__(kHcThreads, 1) sky_hc_kernel(const Params p) { hc_body<kHcDepth, kBlkChk, kLinked, kOpt>(p); }
 
 }  // namespace sky

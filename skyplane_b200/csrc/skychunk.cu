@@ -30,6 +30,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <memory>
 #include <new>
 #include <numeric>
@@ -728,53 +729,38 @@ struct HcArrays {  // SKY_F_HC: the HC kernel's scratch, and the stream the dige
     Stream md5_stream;
     Event ev_fork, ev_join;
 };
-// the HC kernel of each level, kHcMinLevel .. kHcMaxLevel
-using HcKernel = void (*)(const Params);
-static const HcKernel kHcKernels[] = {sky_hc_kernel<hc_depth(3)>, sky_hc_kernel<hc_depth(4)>, sky_hc_kernel<hc_depth(5)>,
-                                      sky_hc_kernel<hc_depth(6)>, sky_hc_kernel<hc_depth(7)>, sky_hc_kernel<hc_depth(8)>,
-                                      sky_hc_kernel<hc_depth(9)>};
-static_assert(sizeof(kHcKernels) / sizeof(kHcKernels[0]) == kHcMaxLevel - kHcMinLevel + 1, "one HC kernel per level");
-// ... and with block checksums (SKY_F_BLOCK_CHECKSUM)
-static const HcKernel kHcBcKernels[] = {sky_hc_bc_kernel<hc_depth(3)>, sky_hc_bc_kernel<hc_depth(4)>, sky_hc_bc_kernel<hc_depth(5)>,
-                                        sky_hc_bc_kernel<hc_depth(6)>, sky_hc_bc_kernel<hc_depth(7)>, sky_hc_bc_kernel<hc_depth(8)>,
-                                        sky_hc_bc_kernel<hc_depth(9)>};
-static_assert(sizeof(kHcBcKernels) == sizeof(kHcKernels), "one HC kernel with block checksums per level");
-// ... and both with linked blocks (SKY_F_LINKED)
-static const HcKernel kHcLinkedKernels[] = {sky_hc_linked_kernel<hc_depth(3)>, sky_hc_linked_kernel<hc_depth(4)>,
-                                            sky_hc_linked_kernel<hc_depth(5)>, sky_hc_linked_kernel<hc_depth(6)>,
-                                            sky_hc_linked_kernel<hc_depth(7)>, sky_hc_linked_kernel<hc_depth(8)>,
-                                            sky_hc_linked_kernel<hc_depth(9)>};
-static const HcKernel kHcLinkedBcKernels[] = {sky_hc_linked_bc_kernel<hc_depth(3)>, sky_hc_linked_bc_kernel<hc_depth(4)>,
-                                              sky_hc_linked_bc_kernel<hc_depth(5)>, sky_hc_linked_bc_kernel<hc_depth(6)>,
-                                              sky_hc_linked_bc_kernel<hc_depth(7)>, sky_hc_linked_bc_kernel<hc_depth(8)>,
-                                              sky_hc_linked_bc_kernel<hc_depth(9)>};
-static_assert(sizeof(kHcLinkedKernels) == sizeof(kHcKernels) && sizeof(kHcLinkedBcKernels) == sizeof(kHcKernels),
-              "one linked HC kernel, with and without block checksums, per level");
-// ... and all four with the optimal parse (SKY_F_OPTIMAL)
-static const HcKernel kHcOptKernels[] = {sky_hc_opt_kernel<hc_depth(3)>, sky_hc_opt_kernel<hc_depth(4)>, sky_hc_opt_kernel<hc_depth(5)>,
-                                         sky_hc_opt_kernel<hc_depth(6)>, sky_hc_opt_kernel<hc_depth(7)>, sky_hc_opt_kernel<hc_depth(8)>,
-                                         sky_hc_opt_kernel<hc_depth(9)>};
-static const HcKernel kHcOptBcKernels[] = {sky_hc_opt_bc_kernel<hc_depth(3)>, sky_hc_opt_bc_kernel<hc_depth(4)>,
-                                           sky_hc_opt_bc_kernel<hc_depth(5)>, sky_hc_opt_bc_kernel<hc_depth(6)>,
-                                           sky_hc_opt_bc_kernel<hc_depth(7)>, sky_hc_opt_bc_kernel<hc_depth(8)>,
-                                           sky_hc_opt_bc_kernel<hc_depth(9)>};
-static const HcKernel kHcOptLinkedKernels[] = {sky_hc_opt_linked_kernel<hc_depth(3)>, sky_hc_opt_linked_kernel<hc_depth(4)>,
-                                               sky_hc_opt_linked_kernel<hc_depth(5)>, sky_hc_opt_linked_kernel<hc_depth(6)>,
-                                               sky_hc_opt_linked_kernel<hc_depth(7)>, sky_hc_opt_linked_kernel<hc_depth(8)>,
-                                               sky_hc_opt_linked_kernel<hc_depth(9)>};
-static const HcKernel kHcOptLinkedBcKernels[] = {sky_hc_opt_linked_bc_kernel<hc_depth(3)>, sky_hc_opt_linked_bc_kernel<hc_depth(4)>,
-                                                 sky_hc_opt_linked_bc_kernel<hc_depth(5)>, sky_hc_opt_linked_bc_kernel<hc_depth(6)>,
-                                                 sky_hc_opt_linked_bc_kernel<hc_depth(7)>, sky_hc_opt_linked_bc_kernel<hc_depth(8)>,
-                                                 sky_hc_opt_linked_bc_kernel<hc_depth(9)>};
-static_assert(sizeof(kHcOptKernels) == sizeof(kHcKernels) && sizeof(kHcOptBcKernels) == sizeof(kHcKernels) &&
-              sizeof(kHcOptLinkedKernels) == sizeof(kHcKernels) && sizeof(kHcOptLinkedBcKernels) == sizeof(kHcKernels),
-              "one optimal-parse HC kernel of each kind per level");
+using Kernel = void (*)(const Params);
+// The fused kernel a batch runs, by [SKY_F_CHECKSUM][SKY_F_BLOCK_CHECKSUM].
+static constexpr Kernel kFusedKernels[2][2] = {{sky_fused_kernel, sky_fused_bc_kernel}, {sky_fused_xxh_kernel, sky_fused_xxh_bc_kernel}};
 constexpr uint32_t kHcLevelShift = 8, kHcLevelMask = 0xfu << kHcLevelShift;  // SKY_F_HC_LEVEL's field in `flags`
 static_assert(SKY_F_HC_LEVEL(1) == (SKY_F_HC | (1u << kHcLevelShift)), "the level field of include/skychunk.h");
 // The level a batch's flags select: the level field, or kHcDefaultLevel when it is 0.
 static int hc_level(uint32_t flags) {
     const int l = (int)((flags & kHcLevelMask) >> kHcLevelShift);
     return l ? l : kHcDefaultLevel;
+}
+// Every HC kernel with the dynamic shared memory it is launched with: entry (row * kHcLevels + level - kHcMinLevel),
+// where row's bits 2, 1, 0 are SKY_F_BLOCK_CHECKSUM, SKY_F_LINKED and SKY_F_OPTIMAL.
+struct HcKernel {
+    Kernel kernel;
+    uint32_t smem;
+};
+constexpr int kHcLevels = kHcMaxLevel - kHcMinLevel + 1;
+static_assert(kHcMinLevel >= 1 && kHcLevels >= 1 && kHcMaxLevel <= (int)(kHcLevelMask >> kHcLevelShift),
+              "the HC levels are a range the level field can hold");
+template <int I>
+static constexpr HcKernel hc_kernel_at() {
+    constexpr int row = I / kHcLevels;
+    constexpr bool bc = row & 4, linked = row & 2, opt = row & 1;
+    return {sky_hc_kernel<hc_depth(kHcMinLevel + I % kHcLevels), bc, linked, opt>, linked ? kHcLinkedSmemBytes : kHcSmemBytes};
+}
+template <int... I>
+static constexpr std::array<HcKernel, sizeof...(I)> hc_kernels(std::integer_sequence<int, I...>) { return {hc_kernel_at<I>()...}; }
+static constexpr std::array<HcKernel, 8 * kHcLevels> kHcKernels = hc_kernels(std::make_integer_sequence<int, 8 * kHcLevels>{});
+// The HC kernel a batch's flags select (SKY_F_HC, its level checked by frame_flags_valid).
+static const HcKernel &hc_kernel(uint32_t flags) {
+    const int row = (flags & SKY_F_BLOCK_CHECKSUM ? 4 : 0) | (flags & SKY_F_LINKED ? 2 : 0) | (flags & SKY_F_OPTIMAL ? 1 : 0);
+    return kHcKernels[row * kHcLevels + hc_level(flags) - kHcMinLevel];
 }
 struct BlockTable {  // per block of a batch, `cap` entries: what frame_index found; done = decoded (the receiver's MD5 gate)
     DevMem<DecBlock> blocks; DevMem<uint32_t> done; uint64_t cap = 0;
@@ -1053,30 +1039,14 @@ int sky_ctx_create(int device, uint64_t max_batch_bytes, uint32_t max_chunks, ui
     ctx->out_cap = max_batch_bytes + (uint64_t)max_chunks * (64 + 4 * 3) + 8 * (max_batch_bytes / kBlock + 1) + 256;
     CK(ctx, cudaSetDevice(device));
     CK(ctx, cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
-    cudaError_t e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_xxh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(sky_fused_xxh_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    for (const auto k : {sky_fused_bc_kernel, sky_fused_xxh_bc_kernel}) {
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    }
-    for (const HcKernel k : kHcKernels)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
-    for (const HcKernel k : kHcBcKernels)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
-    for (const HcKernel k : kHcLinkedKernels)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcLinkedSmemBytes);
-    for (const HcKernel k : kHcLinkedBcKernels)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcLinkedSmemBytes);
-    for (const HcKernel k : kHcOptKernels)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
-    for (const HcKernel k : kHcOptBcKernels)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmemBytes);
-    for (const HcKernel k : kHcOptLinkedKernels)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcLinkedSmemBytes);
-    for (const HcKernel k : kHcOptLinkedBcKernels)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcLinkedSmemBytes);
+    cudaError_t e = cudaSuccess;
+    for (const auto &row : kFusedKernels)
+        for (const Kernel k : row) {
+            if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+            if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+        }
+    for (const HcKernel &k : kHcKernels)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem);
     if (e != cudaSuccess) {
         g_err = ctx->err = std::string("cudaFuncSetAttribute(smem): ") + cudaGetErrorString(e) + " (this build carries sm_90a code only)";
         return SKY_E_CUDA;
@@ -1322,25 +1292,18 @@ static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t met
             CK(ctx, cudaStreamWaitEvent(h.md5_stream, h.ev_fork, 0));
             Params pm = p;
             pm.flags = SKY_F_MD5;
-            if (xxh) sky_fused_xxh_kernel<<<grid, kThreads, kSmemBytes, h.md5_stream>>>(pm);
-            else sky_fused_kernel<<<grid, kThreads, kSmemBytes, h.md5_stream>>>(pm);
+            kFusedKernels[xxh][false]<<<grid, kThreads, kSmemBytes, h.md5_stream>>>(pm);
             CK(ctx, cudaGetLastError());
             CK(ctx, cudaEventRecord(h.ev_join, h.md5_stream));
             ctx->launches++;
         }
         p.scratch = h.scratch;
-        const int lv = hc_level(flags) - kHcMinLevel;
-        const bool opt = (flags & SKY_F_OPTIMAL) != 0;
-        if (flags & SKY_F_LINKED)
-            (opt ? (bc ? kHcOptLinkedBcKernels : kHcOptLinkedKernels) : (bc ? kHcLinkedBcKernels : kHcLinkedKernels))[lv]<<<
-                ctx->sm_count, kHcThreads, kHcLinkedSmemBytes, st>>>(p);
-        else
-            (opt ? (bc ? kHcOptBcKernels : kHcOptKernels) : (bc ? kHcBcKernels : kHcKernels))[lv]<<<ctx->sm_count, kHcThreads, kHcSmemBytes, st>>>(p);
+        const HcKernel &k = hc_kernel(flags);
+        k.kernel<<<ctx->sm_count, kHcThreads, k.smem, st>>>(p);
         CK(ctx, cudaGetLastError());
         if (md5) CK(ctx, cudaStreamWaitEvent(st, h.ev_join, 0));
     } else {
-        void (*const k)(const Params) = bc ? (xxh ? sky_fused_xxh_bc_kernel : sky_fused_bc_kernel) : (xxh ? sky_fused_xxh_kernel : sky_fused_kernel);
-        k<<<grid, kThreads, kSmemBytes, st>>>(p);
+        kFusedKernels[xxh][bc]<<<grid, kThreads, kSmemBytes, st>>>(p);
         CK(ctx, cudaGetLastError());
     }
     ctx->launches++;

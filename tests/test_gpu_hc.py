@@ -71,12 +71,15 @@ def twin_set():
     return datas
 
 
-def check_frame(frame: bytes, data: bytes):
+def check_frame(frame: bytes, data: bytes, block_checksum: bool = False, linked: bool = False):
+    """block_checksum: the frame has 4 more bytes per block, and the strict oracle decoder, which takes no checksums,
+    does not read it; linked: a frame of more than one block has B.Indep clear."""
     n = len(data)
-    assert len(frame) <= native.frame_bound(n)
-    out, info = oracle.lz4f_decode(frame, n, with_info=True)
-    assert out == data and info["consumed"] == len(frame)
-    assert info["bd"] == 0x40 and info["flg"] == (0x68 if n else 0x60)
+    assert len(frame) <= native.frame_bound(n) + (4 * -(-n // 65536) if block_checksum else 0)
+    assert frame[5] == 0x40 and frame[4] == (0x68 if n else 0x60) & ~(0x20 if linked and n > 65536 else 0) | (0x10 if block_checksum else 0)
+    if not block_checksum:
+        out, info = oracle.lz4f_decode(frame, n, with_info=True)
+        assert out == data and info["consumed"] == len(frame)
     assert ref.lz4f_decompress(frame, n) == data
 
 

@@ -1,9 +1,10 @@
 """GPU tests of the high-ratio levels (SKY_F_HC_LEVEL(3..9), python-lz4's compression_level) through the C ABI, ChunkStage
 and GatewayCompressHash.
 
-Bars: at every level the frames are byte-identical to the sequential twin (tools/lz4hc_model.c) at depth 2^(level-1); MD5
-bit-exact; every frame decodes with the strict oracle decoder, liblz4 and sky_decode; SKY_F_HC_LEVEL(5) is SKY_F_HC; on
-16 x 16 MiB Silesia-like chunks level 3 < 5 < 9 in ratio, and level 9 >= 1.02 x level 5.
+Bars: at every level, with and without block checksums, linked blocks and the optimal parse, the frames are
+byte-identical to the sequential twin (tools/lz4hc_model.c) at depth 2^(level-1); MD5 bit-exact; every frame decodes with
+the strict oracle decoder (without block checksums), liblz4 and sky_decode; SKY_F_HC_LEVEL(5) is SKY_F_HC; on 16 x 16 MiB
+Silesia-like chunks level 3 < 5 < 9 in ratio, and level 9 >= 1.02 x level 5.
 """
 import hashlib
 import json
@@ -80,17 +81,26 @@ def datas():
     return twin_set()
 
 
-@pytest.mark.parametrize("level", list(LEVELS))
-def test_frames_equal_twin_at_every_level(ctx, stage, datas, level):
-    """The kernel at each level is pinned to the sequential twin at depth 2^(level-1) byte for byte; every frame decodes
-    with the oracle and liblz4, and sky_decode restores the chunks with the sender's digests."""
+# every HC kernel: id "<level>" is the plain frame, and each option adds its suffix ("5-bc-linked-opt")
+HC_KERNELS = [pytest.param(level, bc, linked, optimal,
+                           id="-".join([str(level)] + [s for s, on in (("bc", bc), ("linked", linked), ("opt", optimal)) if on]))
+              for level in LEVELS for bc in (False, True) for linked in (False, True) for optimal in (False, True)]
+
+
+@pytest.mark.parametrize("level,bc,linked,optimal", HC_KERNELS)
+def test_frames_equal_twin_at_every_level(ctx, stage, datas, level, bc, linked, optimal):
+    """Every HC kernel -- each level with and without block checksums, linked blocks and the optimal parse -- is pinned
+    to the sequential twin at depth 2^(level-1) byte for byte; every frame decodes with liblz4 (and the oracle when it
+    has no block checksums), and sky_decode restores the chunks with the sender's digests."""
     o = twin_opts(level)
-    frames, digests, lens = run_device(ctx, datas, native.hc_level_flag(level) | STAGES)
+    flags = native.hc_level_flag(level) | STAGES
+    flags |= (native.F_BLOCK_CHECKSUM if bc else 0) | (native.F_LINKED if linked else 0) | (native.F_OPTIMAL if optimal else 0)
+    frames, digests, lens = run_device(ctx, datas, flags, extra=4 * -(-max(map(len, datas)) // 65536) if bc else 0)
     for i, (d, f, dg, ln) in enumerate(zip(datas, frames, digests, lens)):
-        want = hm.frame(d, o)
-        assert f == want, f"level {level} chunk {i} (len {len(d)}): GPU frame {len(f)} B != twin {len(want)} B"
+        want = hm.frame(d, o, block_checksum=bc, linked=linked, optimal=optimal, seg=native.kernel_config()["hc_opt_seg"])
+        assert f == want, f"level {level} flags {flags:#x} chunk {i} (len {len(d)}): GPU frame {len(f)} B != twin {len(want)} B"
         assert ln == len(f) and dg == hashlib.md5(d).digest()
-        check_frame(f, d)
+        check_frame(f, d, block_checksum=bc, linked=linked)
     out = stage.decode(frames, [len(d) for d in datas])
     for d, (data, dg, st) in zip(datas, out):
         assert st == 0 and data == d and dg == hashlib.md5(d).digest()
