@@ -9,6 +9,9 @@ decode to come from the generator itself, which builds the output and the sequen
     short).  ``conforming`` streams keep LZ4's end-of-block rules (the last 5 bytes of a block are literals, the last
     match starts at least 12 bytes before the block end), so liblz4 accepts them; ``lenient`` streams end every
     compressed block with a sequence that breaks one of those rules, which liblz4 rejects in a full-size block.
+  * ``conforms`` walks a frame's blocks (``walk_block``) for the receiver's layout, nonzero offsets and the end-of-block
+    rules in every block, short ones too; ``short_block_cases`` makes short last blocks that break those rules and that
+    liblz4 still decodes.
   * the mutators change one structural thing: a header field, a block word, a token, an extension byte, an offset,
     the EndMark, a checksum, whole blocks, or the frame's length.
 """
@@ -342,6 +345,82 @@ def gen_stream(rng: random.Random, size: int, linked: bool = False, conforming: 
             violations.append(j)
     assert len(buf) == size
     return Stream(bytes(buf), blocks, linked, conforming, violations)
+
+
+def short_block_cases(rng: random.Random, head: bytes, want: int) -> List[Tuple[str, Block, bytes]]:
+    """Last blocks of `want` (400 .. 65000) bytes behind the stream `head` that break an end-of-block rule: a 300-byte last
+    match followed by 3 or 4 literals, and a 4-byte last match that starts 9, 10 or 11 bytes before the block end.  liblz4
+    enforces these rules in blocks of (nearly) 64 KiB only and decodes all five here (3 literals only behind a match long
+    enough for a length extension).  -> [(name, block, the whole stream's content)]"""
+    assert 400 <= want <= 65000
+    out = []
+    for lits in (3, 4):
+        buf = bytearray(head)
+        w = BlockWriter(buf).literals(rng.randbytes(want - 300 - lits)).match(8, 300).literals(rng.randbytes(lits))
+        out.append((f"long last match, then {lits} literals", w.close(), bytes(buf)))
+    for k in (9, 10, 11):
+        buf = bytearray(head)
+        w = BlockWriter(buf).literals(rng.randbytes(want - k)).match(7, MIN_MATCH).literals(rng.randbytes(k - MIN_MATCH))
+        out.append((f"4-byte match {k} bytes before the end", w.close(), bytes(buf)))
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ end-of-block rules
+def walk_block(block: bytes) -> Tuple[List[Tuple[int, int]], int]:
+    """The sequences of one well-formed LZ4 block -> ([(output position, offset, length) of every match], decoded length)."""
+    def length(i: int, n: int) -> Tuple[int, int]:
+        if n == 15:
+            while block[i] == 255:
+                n += 255
+                i += 1
+            n += block[i]
+            i += 1
+        return i, n
+
+    i = pos = 0
+    matches = []
+    while i < len(block):
+        tok = block[i]
+        i, ll = length(i + 1, tok >> 4)
+        i += ll
+        pos += ll
+        if i >= len(block):
+            break
+        off = block[i] | block[i + 1] << 8
+        i, ml = length(i + 2, tok & 15)
+        matches.append((pos, off, ml + MIN_MATCH))
+        pos += ml + MIN_MATCH
+    return matches, pos
+
+
+def conforms(frame: bytes, n: int) -> bool:
+    """Does a well-formed frame of an n-byte chunk keep the stage's block layout and LZ4's block rules?  Every block decodes
+    to min(64 KiB, n - its start) bytes, and in every compressed block each match has an offset of at least 1, starts at
+    least MF_LIMIT bytes before the block's end and leaves at least LAST_LITERALS literals behind it -- relative to the
+    block's own decoded length, so in a short last block too.  liblz4 asks for the end-of-block rules in full blocks only,
+    and takes offset 0 as a copy of whatever its output buffer holds there."""
+    try:
+        flg = frame[4]
+        ip, pos = header_len(flg), 0
+        while True:
+            w = struct.unpack_from("<I", frame, ip)[0]
+            ip += 4
+            if w == 0:
+                return pos == n
+            size, want = w & 0x7FFFFFFF, min(BLOCK, n - pos)
+            if want <= 0 or ip + size > len(frame):
+                return False
+            if w & 0x80000000:
+                if size != want:
+                    return False
+            else:
+                matches, out = walk_block(frame[ip : ip + size])
+                if out != want or any(off == 0 or q + MF_LIMIT > want or q + ml > want - LAST_LITERALS for q, off, ml in matches):
+                    return False
+            pos += want
+            ip += size + (4 if flg & FLG_BLOCK_CHK else 0)
+    except (IndexError, struct.error):
+        return False
 
 
 # ------------------------------------------------------------------------------------------------ mutators

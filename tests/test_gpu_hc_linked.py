@@ -3,10 +3,9 @@ ChunkStage and the gateway operators.
 
 Bars: at every level 3..9 the frames are byte-identical to the linked twin (tools/lz4hc_model.c, hc_compress_block_linked)
 on a ragged batch of edge lengths, 8 MiB Silesia-like and text-like chunks, with and without block and content checksums;
-MD5 bit-exact; liblz4 and sky_decode restore every chunk; SKY_F_VERIFY passes clean linked frames unchanged and, through
-sky_verify_device, reports a match before the chunk's first byte as SKY_D_CORRUPT and a changed literal as SKY_D_MISMATCH,
-repairing both into linked stored-block frames; E2EE boxes seal the twin frame; the flag's refusals; run-to-run
-determinism; GatewayCompressHash(compression_level=5, block_linked=True) into GatewayDecompressVerify."""
+MD5 bit-exact; liblz4 and sky_decode restore every chunk; SKY_F_VERIFY passes clean linked frames unchanged (its status
+table, mutants and repair on linked frames are in test_gpu_verify.py); E2EE boxes seal the twin frame; the flag's
+refusals; run-to-run determinism; GatewayCompressHash(compression_level=5, block_linked=True) into GatewayDecompressVerify."""
 import hashlib
 import json
 import os
@@ -17,13 +16,11 @@ from pathlib import Path
 
 import pytest
 
-import lz4_craft as C
 import oracle
 import oracle.reflib as ref
 from skyplane_b200 import native, synth
 from skyplane_b200.stage import ChunkStage
 from test_gpu_hc_levels import run_device
-from test_gpu_verify import run_verify
 from test_linked_format import text, with_content_checksum
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900, method="thread")]
@@ -31,7 +28,6 @@ pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900, method="thread")]
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 from tools import hc_model as hm  # noqa: E402
-from tools import tile_model  # noqa: E402
 
 LK, BC, CK = native.F_LINKED, native.F_BLOCK_CHECKSUM, native.F_CHECKSUM
 KEY = bytes((13 * i + 7) & 0xFF for i in range(32))
@@ -111,36 +107,6 @@ def test_verify_passes_clean_linked_frames(stage, datas):
         checked = stage.process(datas, verify=True, **kw)
         for d, p, c in zip(datas, plain, checked):
             assert c.verify_status == 0 and bytes(c.frame) == bytes(p.frame) == twin(d, level, ck) and c.md5 == p.md5
-
-
-def _crafted(data: bytes):
-    """Linked frames of `data` (three blocks, period 40000, so block 1 is one match reaching 40000 bytes back): a good one,
-    one whose block 0 reaches before the chunk's first byte, one with a changed literal in block 1."""
-    blk = [data[i : i + 65536] for i in range(0, len(data), 65536)]
-    b1 = C.encode_block([(b"", 40000, 65536 - 5)], blk[1][-5:])
-    good = C.assemble_frame([C.stored_block(blk[0]), b1, C.stored_block(blk[2])], data, linked=True, content_size=True)
-    b0 = C.encode_block([(blk[0][:4], 5, 4)], blk[0][8:])
-    before = C.assemble_frame([b0, b1, C.stored_block(blk[2])], data, linked=True, content_size=True)
-    lit = C.flip(good.data, good.spans[1][1] - 1, 0x01)
-    return good.data, before.data, lit
-
-
-def test_verify_device_on_crafted_linked_frames(ctx):
-    data = (synth.random_chunk(9, 40000) * 5)[: 3 * 65536]
-    good, before, lit = _crafted(data)
-    assert ref.lz4f_decompress(good, len(data)) == data
-    flags = native.F_HC | LK
-    st, after, _ = run_verify(ctx, [data] * 3, [good, before, lit], flags, repair=False)
-    assert st == [0, native.D_CORRUPT, native.D_MISMATCH], st
-    # the same match is out of bounds in an independent frame
-    indep = C.with_header(good, flg=good[4] | 0x20)
-    assert run_verify(ctx, [data], [indep], native.F_HC, repair=False)[0] == [native.D_CORRUPT]
-    st, after, flen = run_verify(ctx, [data] * 3, [good, before, lit], flags, repair=True)
-    assert st == [0, native.D_CORRUPT, native.D_MISMATCH]
-    stored = tile_model.assemble(len(data), [(0, b) for b in (data[:65536], data[65536:131072], data[131072:])], linked=True)
-    assert after[0] == good and after[1] == after[2] == stored and stored[4] == 0x48
-    for f in after:
-        assert ref.lz4f_decompress(f, len(data)) == data
 
 
 def test_e2ee_boxes_seal_the_linked_twin_frame(stage):

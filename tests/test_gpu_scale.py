@@ -215,13 +215,16 @@ def _mutate_for_verify(frame, data, k):
     return None
 
 
-def test_verify_at_the_receiver_width(ctx, sm, sources):
+def check_verify_at_the_receiver_width(ctx, sm, sources, linked: bool):
+    """Fast-path frames, or linked high-ratio level-3 frames, of one batch at the receiver's width: all pass, then ~1 % of
+    them mutated fail with the expected codes and are repaired."""
     n = receiver_width(sm)
     assert groups(n) > sm
     datas = ragged_chunks(sources, n, 128 << 10, seed=6)
-    frames, digests, _, _ = run_device(ctx, datas)
+    frames, digests, _, _ = run_device(ctx, datas, LZ4 | MD5 | HC3 | LINKED if linked else 0)
     assert_all(digests, [hashlib.md5(d).digest() for d in datas], "digests")
-    st, _, _ = run_verify(ctx, datas, frames, 0, repair=False)
+    flags = native.F_HC | LINKED if linked else 0
+    st, _, _ = run_verify(ctx, datas, frames, flags, repair=False)
     assert st == [0] * n, [(i, s) for i, s in enumerate(st) if s][:8]
     rng = np.random.default_rng(7)
     mutated, want = list(frames), [0] * n
@@ -234,10 +237,18 @@ def test_verify_at_the_receiver_width(ctx, sm, sources):
             mutated[i], want[i] = m
             k += 1
     assert k == max(1, n // 100)
-    st, _, _ = run_verify(ctx, datas, mutated, 0, repair=False)
+    st, _, _ = run_verify(ctx, datas, mutated, flags, repair=False)
     assert_all(st, want, "statuses")
     assert {native.D_MISMATCH, native.D_CORRUPT} <= set(want)
-    check_repair(ctx, datas, mutated, 0, st)  # failing frames become tile_model.assemble's stored-block frame
+    check_repair(ctx, datas, mutated, flags, st)  # failing frames become tile_model.assemble's stored-block frame
+
+
+def test_verify_at_the_receiver_width(ctx, sm, sources):
+    check_verify_at_the_receiver_width(ctx, sm, sources, linked=False)
+
+
+def test_verify_linked_at_the_receiver_width(ctx, sm, sources):
+    check_verify_at_the_receiver_width(ctx, sm, sources, linked=True)
 
 
 def test_stage_host_path_at_the_receiver_width(sm, sources, twin_opts):

@@ -13,6 +13,7 @@ from types import SimpleNamespace
 import numpy as np
 import pytest
 
+import lz4_craft as C
 import oracle
 import oracle.reflib as ref
 from skyplane_b200 import native, synth
@@ -63,38 +64,12 @@ def test_segment_sizes_give_valid_frames_and_no_match_crosses_a_segment(seg):
         for c, b in hm.blocks(data, hm.kernel_opts(level=5), linked, optimal=True, seg=seg):
             if not c:
                 continue
-            ms = _matches(b)
-            assert [pos for pos, _ in ms] == [pos for pos, _ in sequences(b)]
-            for pos, ml in ms:
+            ms, _ = C.walk_block(b)
+            assert [(pos, off) for pos, off, _ in ms] == sequences(b)
+            for pos, _, ml in ms:
                 assert pos + ml <= 65536
                 if seg:
                     assert pos // seg == (pos + ml - 1) // seg, (seg, pos, ml)
-
-
-def _matches(block: bytes):
-    """(position in the block, length) of every match of one LZ4 block, in one pass."""
-    def length(i, n):
-        if n == 15:
-            while block[i] == 255:
-                n += 255
-                i += 1
-            n += block[i]
-            i += 1
-        return i, n
-
-    i = pos = 0
-    out = []
-    while i < len(block):
-        tok = block[i]
-        i, ll = length(i + 1, tok >> 4)
-        i += ll
-        pos += ll
-        if i >= len(block):
-            break
-        i, ml = length(i + 2, tok & 15)
-        out.append((pos, ml + 4))
-        pos += ml + 4
-    return out
 
 
 def test_whole_block_segment_is_the_cheapest_parse():

@@ -1,7 +1,8 @@
 """The receiver tests' frame corpus (tests/lz4_craft.py), checked on the CPU before any GPU sees it: generated streams
 decode to the generator's bytes with the strict oracle, conforming ones with liblz4 (and pyarrow where installed),
-lenient ones are rejected by liblz4 where they break an end-of-block rule, and each targeted mutator does what the
-receiver tests' tables assume."""
+lenient ones are rejected by liblz4 where they break an end-of-block rule, each targeted mutator does what the
+receiver tests' tables assume, and the block-rule walker (conforms) passes every frame liblz4 and the twins make and
+refuses the short-block and offset-0 frames liblz4 still decodes."""
 import random
 import struct
 
@@ -142,3 +143,66 @@ def test_random_mutants_are_reproducible_and_structural():
         seen.add(a[0].split(":")[0])
     assert seen >= {"flip", "flip_hc_fixed", "truncate", "trailing", "raw_bit", "size+1", "size-1", "size_65537", "drop", "dup",
                     "splice", "no_end_mark", "swap"}
+
+
+def _twin_and_liblz4_frames():
+    """Frames of edge-length chunks from liblz4 (levels 0 and 9) and the stage's CPU twins (fast, high-ratio lazy and
+    optimal), independent and linked."""
+    import sys
+    from pathlib import Path
+
+    sys.path.insert(0, str(Path(__file__).resolve().parent.parent / "tools"))
+    import hc_model as hm
+    import tile_model
+
+    from skyplane_b200 import synth
+
+    for n in (0, 1, 12, 13, 400, 65535, 65536, 65537, 131072 + 999, 200001):
+        for d in (synth.silesia_like_chunk(n % 89, n), (b"it was the best of times, it was the worst of times; " * (n // 50 + 1))[:n]):
+            yield d, tile_model.frame(d)
+            for linked in (False, True):
+                for level in (0, 9):
+                    yield d, hm.liblz4_frame(d, level, linked=linked)
+                for level in (3, 9):
+                    yield d, hm.frame(d, hm.kernel_opts(level=level), linked=linked)
+                yield d, hm.frame(d, hm.kernel_opts(level=5), linked=linked, optimal=True)
+
+
+def test_end_of_block_walker():
+    """lz4_craft.conforms accepts every frame liblz4 and the twins make and every conforming stream, and rejects every
+    lenient block -- short last blocks too, where liblz4 decodes the five short-block cases -- another layout, and offset 0,
+    which liblz4 decodes where its output buffer happens to hold the right bytes."""
+    for d, f in _twin_and_liblz4_frames():
+        assert ref.lz4f_decompress(f, len(d)) == d and C.conforms(f, len(d)), (len(d), f[4])
+    for s in _streams(True):
+        assert C.conforms(s.frame(content_size=True).data, len(s.content))
+    for s in _streams(False):  # every compressed block of a lenient stream long enough for a match breaks a rule
+        bad = [j for j, b in enumerate(s.blocks) if not b.raw and C.walk_block(b.data)[0]]
+        assert C.conforms(s.frame(block_checksum=True).data, len(s.content)) == (not bad)
+    rng = random.Random(12)
+    for head in (b"", rng.randbytes(C.BLOCK)):
+        for want in (400, 1000, 65000):
+            for name, blk, content in C.short_block_cases(rng, head, want):
+                blocks = ([C.stored_block(head)] if head else []) + [blk]
+                f = C.assemble_frame(blocks, content, linked=bool(head), content_size=True).data
+                assert ref.lz4f_decompress(f, len(content)) == content, name
+                assert oracle.lz4f_decode(f, len(content)) == content, name
+                assert not C.conforms(f, len(content)), name
+    buf = bytearray()  # the same end in a full block: liblz4 rejects it too
+    w = C.BlockWriter(buf).literals(rng.randbytes(C.BLOCK - 304)).match(8, 300).literals(rng.randbytes(4))
+    f = C.assemble_frame([w.close()], bytes(buf), content_size=True).data
+    with pytest.raises(ValueError):
+        ref.lz4f_decompress(f, C.BLOCK)
+    assert not C.conforms(f, C.BLOCK)
+    # layout: a short block before the last, or a block too many, is not the stage's layout
+    c = rng.randbytes(100000)
+    assert not C.conforms(C.assemble_frame([C.stored_block(c[:50000]), C.stored_block(c[50000:])], c).data, len(c))
+    assert C.conforms(C.assemble_frame([C.stored_block(c[:C.BLOCK]), C.stored_block(c[C.BLOCK:])], c).data, len(c))
+    assert not C.conforms(C.assemble_frame([C.stored_block(c[:C.BLOCK]), C.stored_block(c[C.BLOCK:]), C.stored_block(b"")], c).data,
+                          len(c))
+    # offset 0: liblz4 copies what its (zeroed) output buffer holds there, so on zeros it restores the chunk
+    z = bytes(1000)
+    f = C.assemble_frame([C.encode_block([(z[:100], 3, 300)], z[400:])], z, content_size=True)
+    p = f.marks["offset"][0]
+    zero = f.data[:p] + b"\0\0" + f.data[p + 2 :]
+    assert ref.lz4f_decompress(zero, len(z)) == z and C.conforms(f.data, len(z)) and not C.conforms(zero, len(z))
