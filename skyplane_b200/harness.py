@@ -59,22 +59,13 @@ def run_stream(
     warmup_requests: int = 0,
     operator_cls=GatewayCompressHash,
     n_slots: int = 4,
-    high_ratio: bool = False,
-    content_checksum: bool = False,
-    compression_level: Optional[int] = None,
-    block_checksum: bool = False,
-    verify_frames: bool = False,
-    block_linked: bool = False,
-    optimal_parse: bool = False,
-    skip_incompressible: bool = False,
+    **operator_options,
 ) -> Dict:
     """Stream ``n_requests`` chunk requests (recycling ``pool_files`` by hard link) through the operator.
 
     The first ``warmup_requests`` completions are not timed (worker start-up: CUDA context, pinned staging).
-    ``high_ratio``, ``content_checksum``, ``compression_level``, ``block_checksum``, ``verify_frames``, ``block_linked``,
-    ``optimal_parse`` and ``skip_incompressible`` are handed to the operator (GatewayCompressHash's high-ratio frames, frames
-    with LZ4's content checksum, the high-ratio level, frames with LZ4's block checksums, the GPU's check of every frame,
-    linked blocks, the optimal parse, incompressible chunks sent as themselves) when set.
+    ``operator_options`` are handed to ``operator_cls`` as they are (GatewayCompressHash's sender options, e.g.
+    ``high_ratio=True`` or ``compression_level=9``).
     Returns {"wall_s", "bytes", "records": [{chunk_id, pool_index, md5, raw_len, frame_path}], "status": {...},
     "frame_verify": {chunk_id: status of every chunk whose frame failed the check},
     "passed_through": [chunk_id of every chunk sent as itself]}.
@@ -87,14 +78,7 @@ def run_stream(
     op = operator_cls(
         "compress_hash", "local:box", qin, qout, err_ev, err_q, store, n_processes=n_workers,
         max_batch_chunks=max_batch_chunks, max_batch_bytes=max_batch_bytes, n_gpus=n_gpus, keep_frames_on_disk=keep_frames, n_slots=n_slots,
-        **({"high_ratio": True} if high_ratio else {}),
-        **({"content_checksum": True} if content_checksum else {}),
-        **({"compression_level": compression_level} if compression_level is not None else {}),
-        **({"block_checksum": True} if block_checksum else {}),
-        **({"verify_frames": True} if verify_frames else {}),
-        **({"block_linked": True} if block_linked else {}),
-        **({"optimal_parse": True} if optimal_parse else {}),
-        **({"skip_incompressible": True} if skip_incompressible else {}),
+        **operator_options,
     )
     op.start_workers()
     records: List[Dict] = []

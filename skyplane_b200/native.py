@@ -215,6 +215,33 @@ def check_passthrough(compress: bool = True, checksum: bool = False, block_check
         raise ValueError("pass-through does not combine with block checksums: a chunk sent as itself has no LZ4 frame to carry them")
 
 
+def sender_flags(compress: bool = True, encrypt: bool = False, hc: bool = False, level: Optional[int] = None, checksum: bool = False,
+                 block_checksum: bool = False, verify: bool = False, linked: bool = False, optimal: bool = False,
+                 passthrough: bool = False) -> int:
+    """The sky_submit flags of ChunkStage.launch's options, or a ValueError naming the option that breaks one of the
+    sender's rules.  ChunkStage and GatewayCompressHash both ask it, so a bad combination fails when an operator is built or
+    before a batch is staged, not in a worker.  Messages name each option by its program field and stage keyword."""
+    for on, what in ((hc, "high_ratio (hc) selects how frames are compressed"),
+                     (checksum, "content_checksum (checksum) is carried by the LZ4 frame"),
+                     (block_checksum, "block_checksum is carried by the LZ4 frame"),
+                     (verify, "verify_frames (verify) checks the LZ4 frames")):
+        if on and not compress:
+            raise ValueError(f"{what}: it needs compression")
+    if passthrough:
+        check_passthrough(compress, checksum, block_checksum)
+    hc_bits = hc_flags(level, hc, compress)
+    # the fast compressor has neither a linked-block mode (DESIGN §4.2) nor an optimal parse
+    if linked and not hc_bits:
+        raise ValueError("block_linked (linked) is a mode of the high-ratio compressor: it needs high_ratio (hc) or a "
+                         "compression_level of 3..9")
+    if optimal and not hc_bits:
+        raise ValueError("optimal_parse (optimal) is a parse of the high-ratio compressor: it needs high_ratio (hc) or a "
+                         "compression_level of 3..9")
+    return (F_MD5 | (F_LZ4 if compress else 0) | (F_E2EE if encrypt else 0) | hc_bits | (F_CHECKSUM if checksum else 0)
+            | (F_BLOCK_CHECKSUM if block_checksum else 0) | (F_VERIFY if verify else 0) | (F_LINKED if linked else 0)
+            | (F_OPTIMAL if optimal else 0) | (F_PASSTHROUGH if passthrough else 0))
+
+
 _DECODE_ONLY_SUBMIT = ((F_HC, "F_HC"), (HC_LEVEL_MASK, "a high-ratio level"), (F_CHECKSUM, "F_CHECKSUM"),
                        (F_BLOCK_CHECKSUM, "F_BLOCK_CHECKSUM"), (F_VERIFY, "F_VERIFY"), (F_LINKED, "F_LINKED"),
                        (F_OPTIMAL, "F_OPTIMAL"), (F_PASSTHROUGH, "F_PASSTHROUGH"))

@@ -177,32 +177,24 @@ class GatewayCompressHash(GatewayOperator):
         straight from the pinned staging slot (``wire.send_results``: WireProtocolHeader + payload, no intermediate bytes
         object, no frame file) -- the tail of ``GatewaySender.process`` (gateway_operator.py:367-402)."""
         super().__init__(handle, region, input_queue, output_queue, error_event, error_queue, chunk_store, n_processes)
-        self.use_compression = True if use_compression is None else bool(use_compression)
-        if high_ratio and not self.use_compression:
-            raise ValueError("high_ratio selects how chunks are compressed: it needs use_compression")
-        self.high_ratio = bool(high_ratio)
-        if content_checksum and not self.use_compression:
-            raise ValueError("content_checksum is carried by the LZ4 frame: it needs use_compression")
-        self.content_checksum = bool(content_checksum)
-        if block_checksum and not self.use_compression:
-            raise ValueError("block_checksum is carried by the LZ4 frame: it needs use_compression")
-        self.block_checksum = bool(block_checksum)
-        if verify_frames and not self.use_compression:
-            raise ValueError("verify_frames checks the LZ4 frames: it needs use_compression")
-        self.verify_frames = bool(verify_frames)
         from skyplane_b200 import native
 
-        hc_bits = native.hc_flags(compression_level, self.high_ratio, self.use_compression)  # (ValueError on a bad level, here and not in a worker)
-        if block_linked and not hc_bits:
-            raise ValueError("block_linked is a mode of the high-ratio compressor: it needs high_ratio or a compression_level of 3..9")
-        self.block_linked = bool(block_linked)
-        if optimal_parse and not hc_bits:
-            raise ValueError("optimal_parse is a parse of the high-ratio compressor: it needs high_ratio or a compression_level of 3..9")
-        self.optimal_parse = bool(optimal_parse)
-        if skip_incompressible:
-            native.check_passthrough(self.use_compression, self.content_checksum, self.block_checksum)
-        self.skip_incompressible = bool(skip_incompressible)
+        self.use_compression = True if use_compression is None else bool(use_compression)
+        self.high_ratio = bool(high_ratio)
+        self.content_checksum = bool(content_checksum)
         self.compression_level = compression_level
+        self.block_checksum = bool(block_checksum)
+        self.verify_frames = bool(verify_frames)
+        self.block_linked = bool(block_linked)
+        self.optimal_parse = bool(optimal_parse)
+        self.skip_incompressible = bool(skip_incompressible)
+        # ChunkStage.launch's keywords of the options that are set, checked here and not in a worker
+        opts = {"hc": high_ratio, "checksum": content_checksum, "block_checksum": block_checksum, "verify": verify_frames,
+                "linked": block_linked, "optimal": optimal_parse, "passthrough": skip_incompressible}
+        self._stage_opts = {k: True for k, on in opts.items() if on}
+        if compression_level is not None:
+            self._stage_opts["level"] = compression_level
+        native.sender_flags(self.use_compression, **self._stage_opts)
         self.e2ee_key_bytes = e2ee_key_bytes
         self.sink = sink
         # batches in flight per worker: a batch of 8 MiB chunks spends >= 70 ms on the GPU whatever its size (one serial MD5
@@ -345,22 +337,7 @@ class GatewayCompressHash(GatewayOperator):
         if not all([fut.result() for _, fut in jobs]):
             stage.release(slot)
             return False
-        opts = {"hc": True} if self.high_ratio else {}
-        if self.content_checksum:
-            opts["checksum"] = True
-        if self.compression_level is not None:
-            opts["level"] = self.compression_level
-        if self.block_checksum:
-            opts["block_checksum"] = True
-        if self.verify_frames:
-            opts["verify"] = True
-        if self.block_linked:
-            opts["linked"] = True
-        if self.optimal_parse:
-            opts["optimal"] = True
-        if self.skip_incompressible:
-            opts["passthrough"] = True
-        stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None, **opts)
+        stage.launch(slot, compress=self.use_compression, encrypt=self.e2ee_key_bytes is not None, **self._stage_opts)
         return True
 
     def _launch(self, reqs: List[ChunkRequest]):

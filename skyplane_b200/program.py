@@ -26,22 +26,20 @@ from skyplane_b200.operators import GatewayCompressHash, GatewayDecompressVerify
 Factory = Callable[[Dict, Dict], GatewayOperator]
 
 
+# compress_hash fields named as GatewayCompressHash's parameters, handed on when the node has them
+_SENDER_FIELDS = ("high_ratio", "content_checksum", "compression_level", "block_checksum", "verify_frames", "block_linked",
+                  "optimal_parse", "skip_incompressible")
+
+
 def _compress_hash(op: Dict, kw: Dict) -> GatewayOperator:
     return GatewayCompressHash(
         **kw,
         n_processes=op.get("num_gpus", 1),
         use_compression=op.get("compress", True),
-        high_ratio=op.get("high_ratio", False),
-        content_checksum=op.get("content_checksum", False),
-        compression_level=op.get("compression_level"),
-        block_checksum=op.get("block_checksum", False),
-        verify_frames=op.get("verify_frames", False),
-        block_linked=op.get("block_linked", False),
-        optimal_parse=op.get("optimal_parse", False),
-        skip_incompressible=op.get("skip_incompressible", False),
         max_batch_chunks=op.get("max_batch_chunks", 64),
         max_batch_bytes=op.get("max_batch_bytes", 512 << 20),
         n_gpus=op.get("num_gpus"),
+        **{f: op[f] for f in _SENDER_FIELDS if f in op},
     )
 
 

@@ -45,15 +45,6 @@ def _out_room(n: int) -> int:
     return native.round16(native.frame_need(n, checksum=True, block_checksum=True) + native.BOX_OVERHEAD)
 
 
-def _check_hc_modes(linked: bool, optimal: bool, hc_bits: int):
-    """linked=True (F_LINKED) and optimal=True (F_OPTIMAL) need the high-ratio mode: the fast compressor has neither a
-    linked-block mode (DESIGN §4.2) nor an optimal parse."""
-    if linked and not hc_bits:
-        raise ValueError("linked=True is a mode of the high-ratio compressor: it needs hc=True or a level 3..9")
-    if optimal and not hc_bits:
-        raise ValueError("optimal=True is a parse of the high-ratio compressor: it needs hc=True or a level 3..9")
-
-
 class _Slot:
     def __init__(self, in_bytes: int, out_bytes: int):
         self.inp = native.PinnedBuffer(in_bytes)
@@ -196,33 +187,19 @@ class ChunkStage:
         passthrough=True sends every chunk whose frame is not smaller than the chunk as the chunk itself (F_PASSTHROUGH):
         its StageResult has is_compressed=False and, without encrypt, `frame` is the chunk in the input slot, which is not
         copied back from the GPU; with encrypt it is the box of the chunk.  The other chunks' frames are unchanged.  It needs
-        compress=True and refuses checksum and block_checksum, which a chunk sent as itself cannot carry."""
+        compress=True and refuses checksum and block_checksum, which a chunk sent as itself cannot carry.
+        A combination that breaks a rule is a ValueError (native.sender_flags)."""
         if not slot.lens:
             raise ValueError("empty batch")
-        if hc and not compress:
-            raise ValueError("hc=True selects how frames are compressed: it needs compress=True")
-        if checksum and not compress:
-            raise ValueError("checksum=True is carried by the LZ4 frame: it needs compress=True")
-        if block_checksum and not compress:
-            raise ValueError("block_checksum=True is carried by the LZ4 frame: it needs compress=True")
-        if verify and not compress:
-            raise ValueError("verify=True checks the LZ4 frames: it needs compress=True")
-        if passthrough:
-            native.check_passthrough(compress, checksum, block_checksum)
-        hc_bits = native.hc_flags(level, hc, compress)
-        _check_hc_modes(linked, optimal, hc_bits)
-        if hc_bits and not native.kernel_config()["hc_depth"]:
+        flags = native.sender_flags(compress, encrypt, hc, level, checksum, block_checksum, verify, linked, optimal, passthrough)
+        if flags & native.F_HC and not native.kernel_config()["hc_depth"]:
             raise native.SkyChunkError(native.SKY_E_INVALID, f"{native.LIB_PATH.name} was built without the high-ratio kernel (F_HC)")
-        if hc_bits & native.HC_LEVEL_MASK and native.kernel_config()["hc_max_level"] < level:
+        if flags & native.HC_LEVEL_MASK and native.kernel_config()["hc_max_level"] < level:
             raise native.SkyChunkError(native.SKY_E_INVALID, f"{native.LIB_PATH.name} was built without high-ratio level {level}")
         if optimal and not native.kernel_config()["hc_opt_seg"]:
             raise native.SkyChunkError(native.SKY_E_INVALID, f"{native.LIB_PATH.name} was built without the optimal parse (F_OPTIMAL)")
         base_in, base_out = slot.inp.addr, slot.out.addr
         src = [base_in + o for o in slot.in_off]
-        flags = (native.F_MD5 | (native.F_LZ4 if compress else 0) | (native.F_E2EE if encrypt else 0) | hc_bits
-                 | (native.F_CHECKSUM if checksum else 0) | (native.F_BLOCK_CHECKSUM if block_checksum else 0)
-                 | (native.F_VERIFY if verify else 0) | (native.F_LINKED if linked else 0) | (native.F_OPTIMAL if optimal else 0)
-                 | (native.F_PASSTHROUGH if passthrough else 0))
         if encrypt and nonces is None:
             nonces = os.urandom(24 * len(slot.lens))  # what nacl.utils.random(24) draws per message
         if compress or encrypt:
@@ -236,17 +213,9 @@ class ChunkStage:
         return slot
 
     def collect(self, slot: _Slot) -> List[StageResult]:
-        comp, enc = bool(slot.flags & native.F_LZ4), bool(slot.flags & native.F_E2EE)
-        if slot.flags & native.F_PASSTHROUGH:
-            out_lens, digests, verify, compressed, self.last_kernel_ms = self.ctx.wait_ex(slot.ticket)
-            verify = verify or [0] * len(slot.lens)
-        elif slot.flags & native.F_VERIFY:
-            out_lens, digests, verify, self.last_kernel_ms = self.ctx.wait_verify(slot.ticket)
-            compressed = [comp] * len(slot.lens)
-        else:
-            out_lens, digests, self.last_kernel_ms = self.ctx.wait(slot.ticket)
-            verify = [0] * len(slot.lens)
-            compressed = [comp] * len(slot.lens)
+        enc = bool(slot.flags & native.F_E2EE)
+        out_lens, digests, verify, compressed, self.last_kernel_ms = self.ctx.wait_ex(slot.ticket)
+        verify = verify or [0] * len(slot.lens)
         res = []
         for io, o, cl, dg, n, v, c in zip(slot.in_off, slot.out_off, out_lens, digests, slot.lens, verify, compressed):
             payload = slot.out.view[o : o + cl] if (c or enc) else slot.inp.view[io : io + n]
@@ -262,13 +231,8 @@ class ChunkStage:
                 verify: bool = False, linked: bool = False, optimal: bool = False, passthrough: bool = False) -> List[StageResult]:
         """Compress + hash (+ seal) a list of in-memory chunks; payloads are returned as independent bytes (hc, checksum,
         level, block_checksum, verify, linked, optimal, passthrough: see launch)."""
-        if passthrough:
-            native.check_passthrough(compress, checksum, block_checksum)
-        _check_hc_modes(linked, optimal, native.hc_flags(level, hc, compress))  # (bad arguments fail before the first batch)
-        if block_checksum and not compress:
-            raise ValueError("block_checksum=True is carried by the LZ4 frame: it needs compress=True")
-        if verify and not compress:
-            raise ValueError("verify=True checks the LZ4 frames: it needs compress=True")
+        # bad options fail before the first batch
+        native.sender_flags(compress, encrypt, hc, level, checksum, block_checksum, verify, linked, optimal, passthrough)
         out: List[StageResult] = []
         i = 0
         while i < len(chunks):
@@ -280,8 +244,12 @@ class ChunkStage:
             if j == i:
                 self.release(slot)
                 raise native.SkyChunkError(native.SKY_E_CAPACITY, f"chunk of {memoryview(chunks[i]).nbytes} bytes exceeds max_batch_bytes")
-            self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum, level, block_checksum,
-                        verify, linked, optimal, passthrough)
+            try:
+                self.launch(slot, compress, encrypt, nonces[24 * i : 24 * j] if nonces is not None else None, hc, checksum, level,
+                            block_checksum, verify, linked, optimal, passthrough)
+            except Exception:
+                self.release(slot)  # (nothing was submitted: the slot's buffers are idle)
+                raise
             for r in self.collect(slot):
                 out.append(StageResult(frame=memoryview(bytes(r.frame)), md5=r.md5, raw_len=r.raw_len, comp_len=r.comp_len,
                                        is_compressed=r.is_compressed, is_encrypted=r.is_encrypted, verify_status=r.verify_status))
