@@ -87,23 +87,34 @@ HC_KERNELS = [pytest.param(level, bc, linked, optimal,
               for level in LEVELS for bc in (False, True) for linked in (False, True) for optimal in (False, True)]
 
 
-@pytest.mark.parametrize("level,bc,linked,optimal", HC_KERNELS)
-def test_frames_equal_twin_at_every_level(ctx, stage, datas, level, bc, linked, optimal):
-    """Every HC kernel -- each level with and without block checksums, linked blocks and the optimal parse -- is pinned
-    to the sequential twin at depth 2^(level-1) byte for byte; every frame decodes with liblz4 (and the oracle when it
-    has no block checksums), and sky_decode restores the chunks with the sender's digests."""
+def assert_frames_equal_twin(ctx, stage, datas, level, bc, linked, optimal, names=None):
+    """One HC kernel's frames of `datas` against the sequential twin at depth 2^(level-1), byte for byte, with and
+    without SKY_F_VERIFY (the frame check must pass every one unchanged); every frame decodes with liblz4 (and the oracle
+    when it has no block checksums), and sky_decode restores the chunks with the sender's digests.  names[i] names chunk
+    i in a failure."""
     o = twin_opts(level)
     flags = native.hc_level_flag(level) | STAGES
     flags |= (native.F_BLOCK_CHECKSUM if bc else 0) | (native.F_LINKED if linked else 0) | (native.F_OPTIMAL if optimal else 0)
     frames, digests, lens = run_device(ctx, datas, flags, extra=4 * -(-max(map(len, datas)) // 65536) if bc else 0)
     for i, (d, f, dg, ln) in enumerate(zip(datas, frames, digests, lens)):
+        name = names[i] if names else f"chunk {i}"
         want = hm.frame(d, o, block_checksum=bc, linked=linked, optimal=optimal, seg=native.kernel_config()["hc_opt_seg"])
-        assert f == want, f"level {level} flags {flags:#x} chunk {i} (len {len(d)}): GPU frame {len(f)} B != twin {len(want)} B"
+        assert f == want, f"level {level} flags {flags:#x} {name} (len {len(d)}): GPU frame {len(f)} B != twin {len(want)} B"
         assert ln == len(f) and dg == hashlib.md5(d).digest()
         check_frame(f, d, block_checksum=bc, linked=linked)
     out = stage.decode(frames, [len(d) for d in datas])
     for d, (data, dg, st) in zip(datas, out):
         assert st == 0 and data == d and dg == hashlib.md5(d).digest()
+    res = stage.process(datas, level=level, block_checksum=bc, linked=linked, optimal=optimal, verify=True)
+    for i, (f, r) in enumerate(zip(frames, res)):
+        assert r.verify_status == 0 and bytes(r.frame) == f, f"level {level} flags {flags:#x} verify: {names[i] if names else i}"
+
+
+@pytest.mark.parametrize("level,bc,linked,optimal", HC_KERNELS)
+def test_frames_equal_twin_at_every_level(ctx, stage, datas, level, bc, linked, optimal):
+    """Every HC kernel -- each level with and without block checksums, linked blocks and the optimal parse -- is pinned
+    to the sequential twin at depth 2^(level-1) byte for byte (assert_frames_equal_twin)."""
+    assert_frames_equal_twin(ctx, stage, datas, level, bc, linked, optimal)
 
 
 def test_level5_is_the_default_high_ratio_mode(ctx, datas):

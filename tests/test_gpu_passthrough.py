@@ -3,10 +3,13 @@ fast compressor, high-ratio level 5 and high-ratio linked + optimal, each with a
 the same batch submitted without the flag; through ChunkStage; and end to end through GatewayCompressHash and
 GatewayDecompressVerify (chunk files, and a socket sink read the way the reference's receiver reads it)."""
 import ctypes
+import functools
 import hashlib
 import multiprocessing as mp
 import socket
+import sys
 import threading
+from pathlib import Path
 
 import numpy as np
 import pytest
@@ -20,23 +23,67 @@ from skyplane_b200.operators import GatewayCompressHash, GatewayDecompressVerify
 from skyplane_b200.stage import ChunkStage
 from test_linked_format import text
 
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+from tools import hc_model as hm  # noqa: E402
+from tools import tile_model as tm  # noqa: E402
+
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600, method="thread")]
 
 KEY = bytes((11 * i + 5) & 0xFF for i in range(32))
 GUARD = 64
 FILL = 0xA5
 MODES = {"fast": 0, "hc5": native.hc_level_flag(5), "hc-linked-optimal": native.F_HC | native.F_LINKED | native.F_OPTIMAL}
+# the chunks at the pass-through edge, at the end of mixed_batch(): (compressor, chunk length, frame length - chunk length)
+EDGE = [(mode, n, delta) for mode in MODES for n in (65536, 2 * 65536 + 100) for delta in (-1, 0, 1)]
 
 
-def mixed_batch():
-    """Random, Silesia-like, text, empty, 1 B, random at 64 KiB and one byte either side, a chunk whose only compressible
-    part is one block (its frame is smaller), and one whose compressible tail is too short to pay for the frame."""
+def twin_frame_len(mode):
+    """The length of `mode`'s frame of a chunk, from the compressor's sequential twin."""
+    k = native.kernel_config()
+    if mode == "fast":
+        o = tm.kernel_opts(k["lz4_entries"], k["seg_slots"], k["max_step_log"])
+        return lambda d: len(tm.frame(d, o))
+    o = hm.Opts(native.hc_depth(5), k["hc_hash_bits"], k["hc_nice"])
+    both = mode == "hc-linked-optimal"
+    return lambda d: len(hm.frame(d, o, linked=both, optimal=both, seg=k["hc_opt_seg"]))
+
+
+def at_the_edge(rng, mode, n, delta):
+    """A random n-byte chunk with one zero run at offset 1000 whose `mode` frame is n + delta bytes: each byte of the run
+    takes about one byte off the frame, so the run's length is stepped to the frame length wanted."""
+    base, flen = rng.bytes(n), twin_frame_len(mode)
+    z, seen = 300, set()
+    while z not in seen:
+        seen.add(z)
+        d = base[:1000] + bytes(z) + base[1000 + z:]
+        got = flen(d)
+        if got == n + delta:
+            return d
+        z = max(1, z + max(-8, min(8, got - n - delta)))
+    for z in range(max(1, min(seen) - 20), max(seen) + 20):  # the length skips a value near the step: walk the run
+        d = base[:1000] + bytes(z) + base[1000 + z:]
+        if flen(d) == n + delta:
+            return d
+    raise RuntimeError(f"no {n}-byte chunk with a {mode} frame of {n + delta} bytes")
+
+
+@functools.lru_cache(maxsize=None)
+def _mixed_batch():
     rng = np.random.default_rng(17)
     one_block = bytearray(rng.bytes(3 * 65536))
     one_block[65536:131072] = text(65536)
     near_miss = rng.bytes(200000) + bytes(24)
-    return [synth.random_chunk(1, (1 << 20) + 7), synth.silesia_like_chunk(2, (1 << 20) + 333), text(300001), b"", b"\x07",
-            rng.bytes(65535), rng.bytes(65536), rng.bytes(65537), bytes(one_block), near_miss, synth.silesia_like_chunk(3, 65536)]
+    return ([synth.random_chunk(1, (1 << 20) + 7), synth.silesia_like_chunk(2, (1 << 20) + 333), text(300001), b"", b"\x07",
+             rng.bytes(65535), rng.bytes(65536), rng.bytes(65537), bytes(one_block), near_miss, synth.silesia_like_chunk(3, 65536)]
+            + [at_the_edge(rng, *e) for e in EDGE])
+
+
+def mixed_batch():
+    """Random, Silesia-like, text, empty, 1 B, random at 64 KiB and one byte either side, a chunk whose only compressible
+    part is one block (its frame is smaller), one whose compressible tail is too short to pay for the frame, and for each
+    compressor in MODES, at one and at two blocks and a bit, chunks whose frame is one byte shorter than the chunk, as
+    long, and one byte longer (EDGE): the first is sent compressed, the other two pass through."""
+    return list(_mixed_batch())
 
 
 @pytest.fixture(scope="module")
@@ -119,6 +166,8 @@ def test_passthrough_against_the_same_batch_without_the_flag(ctx, mode, e2ee, ve
     base = native.F_LZ4 | native.F_MD5 | MODES[mode] | (native.F_VERIFY if verify else 0)
     nonces = np.random.default_rng(3).bytes(24 * len(datas)) if e2ee else None
     f_lens, _, f_ver, _, frames, _ = run(ctx, datas, base)  # the flag-off frames
+    edge = [(n, delta, fl) for (m, n, delta), fl in zip(EDGE, f_lens[-len(EDGE):]) if m == mode]
+    assert edge and all(fl == n + delta for n, delta, fl in edge), edge
     flags = base | native.F_PASSTHROUGH | (native.F_E2EE if e2ee else 0)
     lens, dg, ver, comp, payloads, guards = run(ctx, datas, flags, nonces)
     assert guards
