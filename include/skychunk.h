@@ -38,7 +38,7 @@ extern "C" {
 #define SKY_API
 #endif
 
-#define SKY_ABI_VERSION 3
+#define SKY_ABI_VERSION 4
 
 /* error codes */
 #define SKY_OK 0
@@ -95,7 +95,7 @@ extern "C" {
  * block and content checksums, and every block decoded against the chunk's bytes under liblz4's rules -- so that a frame
  * the stage returns restores its chunk under any LZ4 decoder.  A frame that fails is rewritten in place as the chunk's
  * stored-block frame (same header and checksum flags, every block stored raw; sky_frame_bound plus the checksum bytes,
- * which dst_cap already holds) and its status (sky_wait_verify) is the failing check's SKY_D_* code.  Alone it means
+ * which dst_cap already holds) and its status (sky_wait's verify[i]) is the failing check's SKY_D_* code.  Alone it means
  * LZ4 + MD5 + verify; without SKY_F_LZ4 (no frame) it is SKY_E_INVALID, and sky_process_device does not take it
  * (sky_verify_device runs the same check over frames in HBM).  Three more launches per batch.  It sits outside the
  * SKY_F_HC_LEVEL field. */
@@ -125,9 +125,9 @@ extern "C" {
  * comes back changes.  For a chunk that passes through: without SKY_F_E2EE out_len[i] = 0 and dst[i] is not written (as
  * with SKY_F_MD5 alone, the caller forwards its own input bytes, and nothing is copied back for it); with SKY_F_E2EE dst[i]
  * holds the SecretBox of the chunk's own bytes and out_len[i] = src_len[i] + SKY_BOX_OVERHEAD.  The digests always come
- * back, and SKY_F_VERIFY's statuses too.  Such a ticket is completed by sky_wait_ex only, whose compressed[i] says which
- * payload each chunk got; sky_wait and sky_wait_verify return SKY_E_INVALID and leave it waitable.  It needs SKY_F_LZ4 (or
- * no stage bit) and combines with SKY_F_HC / SKY_F_HC_LEVEL / SKY_F_LINKED / SKY_F_OPTIMAL, SKY_F_E2EE and SKY_F_VERIFY.
+ * back, and SKY_F_VERIFY's statuses too.  sky_wait's compressed[i] says which payload each chunk got, and the ticket
+ * needs it (see sky_wait).  It needs SKY_F_LZ4 (or no stage bit) and combines with SKY_F_HC / SKY_F_HC_LEVEL /
+ * SKY_F_LINKED / SKY_F_OPTIMAL, SKY_F_E2EE and SKY_F_VERIFY.
  * With SKY_F_MD5 alone, SKY_F_CHECKSUM or SKY_F_BLOCK_CHECKSUM (a raw payload cannot carry the LZ4 checksums) it is
  * SKY_E_INVALID, as it is in sky_process_device, sky_verify_device and sky_decode: the receiver takes the chunks that pass
  * through as it takes SKY_F_MD5's payloads. */
@@ -175,21 +175,18 @@ SKY_API int sky_pinned_free(void *p);
  *   back in dst[i] is the sealed box of the frame (or of the raw chunk when SKY_F_LZ4 is off), out_len[i] = its length
  *   = payload + SKY_BOX_OVERHEAD, dst_cap[i] >= sky_box_bound(src_len[i]); nonces = 24 bytes per chunk chosen by the
  *   caller (nacl.utils.random(24)).  The key is the ctx's (sky_set_e2ee_key; key32 = NULL switches E2EE off).
- * sky_wait: blocks until the batch is done, copies each frame device->host (exact length), and
- *   fills out_len[n], md5[16*n].  kernel_ms (optional) = device time of the fused kernel. */
+ * sky_wait: blocks until the batch is done, copies each frame device->host (exact length), and fills the outputs it is
+ *   given, each optional: out_len[n], md5[16*n]; verify[n] = per chunk 0 (the frame restores the chunk) or the SKY_D_*
+ *   code of the frame as the compressor made it, whose payload is now the stored-block frame (SKY_F_VERIFY);
+ *   compressed[n] = per chunk 1 when its payload is a frame (or the SecretBox of a frame), 0 when it is the chunk itself
+ *   (or the SecretBox of the chunk) -- WireProtocolHeader.is_compressed; without SKY_F_PASSTHROUGH it is 1 exactly when
+ *   the ticket has SKY_F_LZ4.  kernel_ms = device time of the fused kernel.  Two requests are SKY_E_INVALID and leave the
+ *   ticket waitable: verify != NULL on a ticket without SKY_F_VERIFY, and compressed == NULL on a SKY_F_PASSTHROUGH
+ *   ticket (a caller that ignored the bit would label a sealed raw chunk as compressed). */
 SKY_API int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t *src_len, void *const *dst,
                const uint64_t *dst_cap, uint32_t flags, const uint8_t *nonces, uint64_t *ticket);
-SKY_API int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, float *kernel_ms);
-/* sky_wait, plus verify[n]: per chunk 0 (the frame restores the chunk) or the SKY_D_* code of the frame as the compressor
- * made it, whose payload is now the stored-block frame.  verify != NULL needs a ticket submitted with SKY_F_VERIFY
- * (SKY_E_INVALID otherwise, and the ticket stays un-waited); sky_wait also completes such a ticket. */
-SKY_API int sky_wait_verify(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, float *kernel_ms);
-/* sky_wait_verify, plus compressed[n] (required): per chunk 1 when its payload is a frame (or the SecretBox of a frame), 0
- * when it is the chunk itself (or the SecretBox of the chunk) -- WireProtocolHeader.is_compressed.  It completes any
- * ticket: without SKY_F_PASSTHROUGH compressed[i] is 1 exactly when the ticket has SKY_F_LZ4.  verify follows
- * sky_wait_verify's rules. */
-SKY_API int sky_wait_ex(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, uint8_t *compressed,
-                        float *kernel_ms);
+SKY_API int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, uint8_t *compressed,
+                     float *kernel_ms);
 SKY_API int sky_set_e2ee_key(sky_ctx *ctx, const uint8_t *key32);
 SKY_API uint64_t sky_box_bound(uint64_t n); /* sky_frame_bound(n) + SKY_BOX_OVERHEAD */
 
@@ -220,7 +217,7 @@ SKY_API int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, cons
  *     ... | SKY_F_E2EE                SecretBox of the frame          SKY_F_E2EE (with or without the two bits)
  *     SKY_F_MD5 (`compress: false`)   the chunk's own bytes           SKY_F_MD5
  *     SKY_F_MD5 | SKY_F_E2EE          SecretBox of the chunk          SKY_F_MD5 | SKY_F_E2EE
- *     ... | SKY_F_PASSTHROUGH         per chunk, one of the rows      per chunk, by sky_wait_ex's compressed[i]:
+ *     ... | SKY_F_PASSTHROUGH         per chunk, one of the rows      per chunk, by sky_wait's compressed[i]:
  *                                     above (frame or chunk)          the frames' row or the chunks' row
  *
  * SKY_F_E2EE: the payloads are sealed boxes, whose tags are checked and which are opened on the device first (status

@@ -1187,6 +1187,8 @@ static bool frame_flags_valid(uint32_t flags) {
 static uint64_t frame_need(uint64_t n, uint32_t flags) {
     return sky_frame_bound(n) + ((flags & SKY_F_CHECKSUM) ? 4 : 0) + ((flags & SKY_F_BLOCK_CHECKSUM) ? 4 * ((n + kBlock - 1) / kBlock) : 0);
 }
+// No stage bit means LZ4 + MD5.
+static uint32_t with_stages(uint32_t flags) { return (flags & (SKY_F_LZ4 | SKY_F_MD5)) ? flags : flags | SKY_F_LZ4 | SKY_F_MD5; }
 
 // Enqueues the frame check (SKY_F_VERIFY, lz4verify.cuh) of the n chunks in the slot's batch metadata (h_desc / d_desc,
 // the frame lengths in outlen, the content checksums in xxh under SKY_F_CHECKSUM) on `st`: index, block check, settle.
@@ -1232,10 +1234,10 @@ static int launch_verify(sky_ctx *ctx, Slot &s, cudaStream_t st, uint32_t n, uin
 
 // Fills the slot's metadata for a batch and enqueues: meta H2D, counter reset, fused kernel, results D2H.
 // `meta_st`: stream the three small metadata copies ride on (the H2D stream on the host path, so they are
-// never queued behind another batch's frame copies); `st`: the stream the kernel runs on.
+// never queued behind another batch's frame copies); `st`: the stream the kernel runs on.  `flags` has a stage bit
+// (with_stages).
 static int launch_batch(sky_ctx *ctx, Slot &s, cudaStream_t st, cudaStream_t meta_st, uint32_t n, const uint8_t *d_src,
                         const uint64_t *src_off, const uint64_t *src_len, uint8_t *d_dst, const uint64_t *dst_off, uint32_t flags) {
-    if ((flags & (SKY_F_LZ4 | SKY_F_MD5)) == 0) flags |= SKY_F_LZ4 | SKY_F_MD5;
     if (flags & SKY_F_CHECKSUM) flags |= SKY_F_MD5;  // the content checksum comes from the MD5 lanes
     const bool xxh = (flags & SKY_F_CHECKSUM) != 0, bc = (flags & SKY_F_BLOCK_CHECKSUM) != 0;
     if (flags & SKY_F_HC) {
@@ -1356,6 +1358,25 @@ static int progress(sky_ctx *ctx) {
     return SKY_OK;
 }
 
+// The synchronous calls run on slot 0 (its metadata, and its slabs for sky_decode): take_slot0 selects the device and
+// the stream (the caller's, or the slot's when NULL) and refuses while the slot holds a ticket; finish_sync waits for
+// the stream and reads kernel_ms (optional) from `start` (the slot's ev_k0 when NULL) to ev_k1.
+static int take_slot0(sky_ctx *ctx, void *stream, cudaStream_t &st) {
+    CK(ctx, cudaSetDevice(ctx->device));
+    Slot &s = ctx->slots[0];
+    if (s.ticket.busy) return SKY_E_BUSY;
+    st = stream ? (cudaStream_t)stream : s.stream;
+    return SKY_OK;
+}
+static int finish_sync(sky_ctx *ctx, cudaStream_t st, float *kernel_ms, cudaEvent_t start = nullptr) {
+    const Slot &s = ctx->slots[0];
+    CK(ctx, cudaStreamSynchronize(st));
+    if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, start ? start : (cudaEvent_t)s.ev_k0, s.ev_k1));
+    return SKY_OK;
+}
+// Device chunk base + off is 16-byte aligned (base and off both are): the kernels move 16 bytes at a time.
+static bool aligned16(const void *base, uint64_t off) { return ((reinterpret_cast<uintptr_t>(base) | off) & 15) == 0; }
+
 int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64_t *src_off, const uint64_t *src_len,
                        void *d_dst, const uint64_t *dst_off, const uint64_t *dst_cap, uint32_t flags, void *stream,
                        uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
@@ -1363,29 +1384,27 @@ int sky_process_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64
     if (flags & (SKY_F_E2EE | SKY_F_VERIFY | SKY_F_PASSTHROUGH)) return SKY_E_INVALID;  // host-path features (sky_submit; sky_verify_device checks)
     if (!frame_flags_valid(flags)) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
-    if ((reinterpret_cast<uintptr_t>(d_src) & 15) || (reinterpret_cast<uintptr_t>(d_dst) & 15)) return SKY_E_INVALID;
     for (uint32_t i = 0; i < n; i++) {
-        if ((src_off[i] & 15) || (dst_off[i] & 15)) return SKY_E_INVALID;
+        if (!aligned16(d_src, src_off[i]) || !aligned16(d_dst, dst_off[i])) return SKY_E_INVALID;
         if (dst_cap[i] < frame_need(src_len[i], flags)) return SKY_E_CAPACITY;
         if (src_len[i] && !d_src) return SKY_E_INVALID;
     }
-    CK(ctx, cudaSetDevice(ctx->device));
-    Slot &s = ctx->slots[0];
-    if (s.ticket.busy) return SKY_E_BUSY;
-    cudaStream_t st = stream ? (cudaStream_t)stream : s.stream;
-    int rc = launch_batch(ctx, s, st, st, n, (const uint8_t *)d_src, src_off, src_len, (uint8_t *)d_dst, dst_off, flags);
+    cudaStream_t st;
+    int rc = take_slot0(ctx, stream, st);
     if (rc != SKY_OK) return rc;
-    CK(ctx, cudaStreamSynchronize(st));
+    Slot &s = ctx->slots[0];
+    rc = launch_batch(ctx, s, st, st, n, (const uint8_t *)d_src, src_off, src_len, (uint8_t *)d_dst, dst_off, with_stages(flags));
+    if (rc == SKY_OK) rc = finish_sync(ctx, st, kernel_ms);
+    if (rc != SKY_OK) return rc;
     if (out_len) memcpy(out_len, s.meta.outlen.h, n * sizeof(uint64_t));
     if (md5) memcpy(md5, s.meta.md5.h, (size_t)n * 16);
-    if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, s.ev_k0, s.ev_k1));
     return SKY_OK;
 }
 
 int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t *src_len, void *const *dst,
                const uint64_t *dst_cap, uint32_t flags, const uint8_t *nonces, uint64_t *ticket) {
     if (!ctx || n == 0 || !src || !src_len || !ticket || !frame_flags_valid(flags)) return SKY_E_INVALID;
-    if ((flags & (SKY_F_LZ4 | SKY_F_MD5)) == 0) flags |= SKY_F_LZ4 | SKY_F_MD5;
+    flags = with_stages(flags);
     const bool e2ee = (flags & SKY_F_E2EE) != 0, frames = (flags & SKY_F_LZ4) != 0;
     const bool returns_data = frames || e2ee;  // MD5-only without E2EE: only digests come back
     if (returns_data && (!dst || !dst_cap)) return SKY_E_INVALID;
@@ -1426,10 +1445,7 @@ int sky_submit(sky_ctx *ctx, uint32_t n, const void *const *src, const uint64_t 
     return SKY_OK;
 }
 
-// The waits: sky_wait_ex (compressed != NULL) completes any ticket; sky_wait and sky_wait_verify (compressed == NULL) refuse
-// a SKY_F_PASSTHROUGH ticket, whose payloads are not all frames.
-static int wait_ticket(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, uint8_t *compressed,
-                       float *kernel_ms) {
+int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, uint8_t *compressed, float *kernel_ms) {
     if (!ctx) return SKY_E_INVALID;
     Slot *sp = nullptr;
     for (Slot &s : ctx->slots)
@@ -1461,19 +1477,6 @@ static int wait_ticket(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t
     return SKY_OK;
 }
 
-int sky_wait_verify(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, float *kernel_ms) {
-    return wait_ticket(ctx, ticket, out_len, md5, verify, nullptr, kernel_ms);
-}
-
-int sky_wait(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, float *kernel_ms) {
-    return wait_ticket(ctx, ticket, out_len, md5, nullptr, nullptr, kernel_ms);
-}
-
-int sky_wait_ex(sky_ctx *ctx, uint64_t ticket, uint64_t *out_len, uint8_t *md5, int32_t *verify, uint8_t *compressed, float *kernel_ms) {
-    if (!compressed) return SKY_E_INVALID;
-    return wait_ticket(ctx, ticket, out_len, md5, verify, compressed, kernel_ms);
-}
-
 int sky_verify_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64_t *src_off, const uint64_t *src_len, void *d_frames,
                       const uint64_t *frame_off, uint64_t *frame_len, const uint64_t *frame_cap, const uint32_t *content_xxh,
                       uint32_t flags, void *stream, int32_t *status, float *kernel_ms) {
@@ -1482,19 +1485,18 @@ int sky_verify_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64_
         return SKY_E_INVALID;
     if (((flags & SKY_F_CHECKSUM) != 0) != (content_xxh != nullptr)) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
-    if (reinterpret_cast<uintptr_t>(d_src) & 15) return SKY_E_INVALID;
     for (uint32_t i = 0; i < n; i++) {
-        if (src_off[i] & 15) return SKY_E_INVALID;
+        if (!aligned16(d_src, src_off[i])) return SKY_E_INVALID;
         if (src_len[i] && !d_src) return SKY_E_INVALID;
         if (frame_cap && frame_cap[i] < frame_need(src_len[i], flags)) return SKY_E_CAPACITY;
     }
-    CK(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st;
+    int rc = take_slot0(ctx, stream, st);
+    if (rc != SKY_OK) return rc;
     Slot &s = ctx->slots[0];
-    if (s.ticket.busy) return SKY_E_BUSY;
-    cudaStream_t st = stream ? (cudaStream_t)stream : s.stream;
     BatchMeta &m = s.meta;
     uint32_t rows;
-    int rc = batch_geometry(n, src_len, rows, [&](uint32_t i, uint32_t nblk) {
+    rc = batch_geometry(n, src_len, rows, [&](uint32_t i, uint32_t nblk) {
         m.h_desc[i] = ChunkDesc{(const uint8_t *)d_src + src_off[i], (uint8_t *)d_frames + frame_off[i], src_len[i], nblk};
     });
     if (rc != SKY_OK) return rc;
@@ -1506,10 +1508,10 @@ int sky_verify_device(sky_ctx *ctx, uint32_t n, const void *d_src, const uint64_
     rc = launch_verify(ctx, s, st, n, rows, flags, frame_cap != nullptr);
     if (rc != SKY_OK) return rc;
     CK(ctx, cudaEventRecord(s.ev_k1, st));
-    CK(ctx, cudaStreamSynchronize(st));
+    rc = finish_sync(ctx, st, kernel_ms);
+    if (rc != SKY_OK) return rc;
     if (status) memcpy(status, s.verify.status.h, n * sizeof(int32_t));
     memcpy(frame_len, m.outlen.h, n * sizeof(uint64_t));
-    if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, s.ev_k0, s.ev_k1));
     return SKY_OK;
 }
 
@@ -1592,21 +1594,19 @@ int sky_decode_device(sky_ctx *ctx, uint32_t n, const void *d_frames, const uint
                       float *kernel_ms) {
     if (!ctx || n == 0 || !d_frames || !frame_off || !frame_len || !out_off || !raw_len) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
-    if (reinterpret_cast<uintptr_t>(d_out) & 15) return SKY_E_INVALID;
     for (uint32_t i = 0; i < n; i++) {
-        if (out_off[i] & 15) return SKY_E_INVALID;
+        if (!aligned16(d_out, out_off[i])) return SKY_E_INVALID;
         if (raw_len[i] && !d_out) return SKY_E_INVALID;
     }
-    CK(ctx, cudaSetDevice(ctx->device));
-    Slot &s = ctx->slots[0];
-    if (s.ticket.busy) return SKY_E_BUSY;
-    cudaStream_t st = stream ? (cudaStream_t)stream : s.stream;
-    int rc = launch_decode(ctx, s, st, n, (const uint8_t *)d_frames, frame_off, frame_len, (uint8_t *)d_out, out_off, raw_len);
+    cudaStream_t st;
+    int rc = take_slot0(ctx, stream, st);
     if (rc != SKY_OK) return rc;
-    CK(ctx, cudaStreamSynchronize(st));
+    Slot &s = ctx->slots[0];
+    rc = launch_decode(ctx, s, st, n, (const uint8_t *)d_frames, frame_off, frame_len, (uint8_t *)d_out, out_off, raw_len);
+    if (rc == SKY_OK) rc = finish_sync(ctx, st, kernel_ms);  // index + decode + MD5
+    if (rc != SKY_OK) return rc;
     if (status) memcpy(status, s.dec.h_status, n * sizeof(int32_t));
     if (md5) memcpy(md5, s.meta.md5.h, (size_t)n * 16);
-    if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, s.ev_k0, s.ev_k1));  // index + decode + MD5
     return SKY_OK;
 }
 
@@ -1638,8 +1638,8 @@ static int decode_raw(sky_ctx *ctx, Slot &s, uint32_t n, const void *const *payl
     }
     // (no frames are written without SKY_F_LZ4: the frame slab only lends the descriptors an address)
     int rc = launch_batch(ctx, s, s.stream, s.stream, n, s.d_in, off.data(), md5_len.data(), s.d_out, off.data(), SKY_F_MD5);
+    if (rc == SKY_OK) rc = finish_sync(ctx, s.stream, kernel_ms, e2ee ? (cudaEvent_t)s.box.ev_open : nullptr);  // open + digest
     if (rc != SKY_OK) return rc;
-    CK(ctx, cudaStreamSynchronize(s.stream));
     for (uint32_t i = 0; i < n; i++) {
         int32_t st = msg_len[i] == raw_len[i] ? SKY_D_OK : SKY_D_SIZE;
         if (e2ee && (s.box.h_status[i] != 0 || payload_len[i] < (uint64_t)kBoxOverhead)) st = SKY_D_AUTH;  // never hand its bytes out
@@ -1652,7 +1652,6 @@ static int decode_raw(sky_ctx *ctx, Slot &s, uint32_t n, const void *const *payl
             CK(ctx, cudaMemcpyAsync(dst[i], s.d_in + off[i], raw_len[i], cudaMemcpyDeviceToHost, s.stream));
     }
     if (e2ee) CK(ctx, cudaStreamSynchronize(s.stream));
-    if (kernel_ms) CK(ctx, cudaEventElapsedTime(kernel_ms, e2ee ? (cudaEvent_t)s.box.ev_open : (cudaEvent_t)s.ev_k0, s.ev_k1));  // open + digest
     return SKY_OK;
 }
 
@@ -1663,11 +1662,12 @@ int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64
     const bool returns_data = !raw || e2ee;  // an unsealed raw chunk is only digested: the caller holds its bytes
     if (!ctx || n == 0 || !frames || !frame_len || (returns_data && !dst) || !raw_len) return SKY_E_INVALID;
     if (n > ctx->max_chunks) return SKY_E_CAPACITY;
+    cudaStream_t st;
+    int rc = take_slot0(ctx, nullptr, st);
+    if (rc != SKY_OK) return rc;
     Slot &s = ctx->slots[0];
-    if (s.ticket.busy) return SKY_E_BUSY;
     if (!s.d_in) return SKY_E_INVALID;  // ctx created without slabs
     if (e2ee && !ctx->d_key) return SKY_E_NOKEY;
-    CK(ctx, cudaSetDevice(ctx->device));
     if (raw) return decode_raw(ctx, s, n, frames, frame_len, dst, raw_len, e2ee, status, md5, kernel_ms);
     // roles swap on the way back: frames (<= bound) go into the frame slab, decoded bytes into the input slab
     std::vector<uint64_t> f_off(n), o_off(n), f_len(frame_len, frame_len + n);
@@ -1682,25 +1682,24 @@ int sky_decode(sky_ctx *ctx, uint32_t n, const void *const *frames, const uint64
     if (fp > ctx->out_cap || op > ctx->in_cap) return SKY_E_CAPACITY;
     if (e2ee) {
         // the payloads are boxes (nonce | tag | ciphertext): check the tags, decrypt into the frame slab, then decode as usual
-        int rc = launch_open(ctx, s, n, frames, frame_len, f_off.data(), s.d_out, f_off.data(), f_len.data());
+        rc = launch_open(ctx, s, n, frames, frame_len, f_off.data(), s.d_out, f_off.data(), f_len.data());
         if (rc != SKY_OK) return rc;
     } else {
         for (uint32_t i = 0; i < n; i++)
-            CK(ctx, cudaMemcpyAsync(s.d_out + f_off[i], frames[i], frame_len[i], cudaMemcpyHostToDevice, s.stream));
+            CK(ctx, cudaMemcpyAsync(s.d_out + f_off[i], frames[i], frame_len[i], cudaMemcpyHostToDevice, st));
     }
-    int rc = sky_decode_device(ctx, n, s.d_out, f_off.data(), f_len.data(), s.d_in, o_off.data(), raw_len, s.stream, status, md5, kernel_ms);
+    rc = launch_decode(ctx, s, st, n, s.d_out, f_off.data(), f_len.data(), s.d_in, o_off.data(), raw_len);
+    if (rc == SKY_OK) rc = finish_sync(ctx, st, kernel_ms);  // index + decode + MD5, without the box open
     if (rc != SKY_OK) return rc;
-    if (e2ee) {
-        for (uint32_t i = 0; i < n; i++)
-            if (s.box.h_status[i] != 0 || frame_len[i] < (uint64_t)kBoxOverhead) {  // forged or truncated box: never hand its bytes out
-                s.dec.h_status[i] = SKY_D_AUTH;
-                if (status) status[i] = SKY_D_AUTH;
-            }
-    }
-    for (uint32_t i = 0; i < n; i++)
+    for (uint32_t i = 0; i < n; i++) {
+        if (e2ee && (s.box.h_status[i] != 0 || frame_len[i] < (uint64_t)kBoxOverhead))  // forged or truncated box: never hand its bytes out
+            s.dec.h_status[i] = SKY_D_AUTH;
         if (raw_len[i] && s.dec.h_status[i] == 0)
-            CK(ctx, cudaMemcpyAsync(dst[i], s.d_in + o_off[i], raw_len[i], cudaMemcpyDeviceToHost, s.stream));
-    CK(ctx, cudaStreamSynchronize(s.stream));
+            CK(ctx, cudaMemcpyAsync(dst[i], s.d_in + o_off[i], raw_len[i], cudaMemcpyDeviceToHost, st));
+    }
+    if (status) memcpy(status, s.dec.h_status, n * sizeof(int32_t));
+    if (md5) memcpy(md5, s.meta.md5.h, (size_t)n * 16);
+    CK(ctx, cudaStreamSynchronize(st));
     return SKY_OK;
 }
 

@@ -40,7 +40,7 @@ D_NAMES = {0: "ok", -1: "bad frame header", -2: "corrupt block", -3: "size misma
 ABI_SYMBOLS = (
     "sky_strerror", "sky_last_error", "sky_abi_version", "sky_device_count", "sky_device_pci_bus_id", "sky_kernel_config", "sky_frame_bound",
     "sky_ctx_create", "sky_ctx_destroy", "sky_pinned_alloc", "sky_pinned_free",
-    "sky_submit", "sky_wait", "sky_wait_verify", "sky_wait_ex", "sky_set_e2ee_key", "sky_box_bound", "sky_process_device", "sky_verify_device",
+    "sky_submit", "sky_wait", "sky_set_e2ee_key", "sky_box_bound", "sky_process_device", "sky_verify_device",
     "sky_decode_device", "sky_decode",
     "sky_device_alloc", "sky_device_free", "sky_memcpy_h2d", "sky_memcpy_d2h", "sky_launch_count",
 )
@@ -111,12 +111,8 @@ def lib() -> ctypes.CDLL:
     L.sky_set_e2ee_key.restype = i32
     L.sky_box_bound.argtypes = [u64]
     L.sky_box_bound.restype = u64
-    L.sky_wait.argtypes = [vp, u64, p_u64, vp, ctypes.POINTER(ctypes.c_float)]
+    L.sky_wait.argtypes = [vp, u64, p_u64, vp, ctypes.POINTER(ctypes.c_int32), vp, ctypes.POINTER(ctypes.c_float)]
     L.sky_wait.restype = i32
-    L.sky_wait_verify.argtypes = [vp, u64, p_u64, vp, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_float)]
-    L.sky_wait_verify.restype = i32
-    L.sky_wait_ex.argtypes = [vp, u64, p_u64, vp, ctypes.POINTER(ctypes.c_int32), vp, ctypes.POINTER(ctypes.c_float)]
-    L.sky_wait_ex.restype = i32
     L.sky_process_device.argtypes = [vp, u32, vp, p_u64, p_u64, vp, p_u64, p_u64, u32, vp, p_u64, vp, ctypes.POINTER(ctypes.c_float)]
     L.sky_process_device.restype = i32
     p_i32 = ctypes.POINTER(ctypes.c_int32)
@@ -382,44 +378,31 @@ class Context:
         return t.value
 
     def wait(self, ticket: int):
-        """-> (out_lens: list[int], digests: list[bytes], kernel_ms: float)"""
-        n, _keep, _flags = self._inflight.pop(ticket)
-        out = (ctypes.c_uint64 * n)()
-        md5 = (ctypes.c_ubyte * (16 * n))()
-        ms = ctypes.c_float(0)
-        self._check(lib().sky_wait(self._h, ticket, out, md5, ctypes.byref(ms)))
-        raw = bytes(md5)
-        return list(out), [raw[16 * i : 16 * i + 16] for i in range(n)], ms.value
-
-    def wait_verify(self, ticket: int):
-        """wait() for a ticket submitted with F_VERIFY -> (out_lens, digests, verify, kernel_ms); verify[i] is 0 or the D_*
-        code of chunk i's frame as the compressor made it (its payload is then the stored-block frame)."""
-        n, _keep, _flags = self._inflight[ticket]
-        out = (ctypes.c_uint64 * n)()
-        md5 = (ctypes.c_ubyte * (16 * n))()
-        ver = (ctypes.c_int32 * n)()
-        ms = ctypes.c_float(0)
-        self._check(lib().sky_wait_verify(self._h, ticket, out, md5, ver, ctypes.byref(ms)))
-        del self._inflight[ticket]
-        raw = bytes(md5)
-        return list(out), [raw[16 * i : 16 * i + 16] for i in range(n)], list(ver), ms.value
+        """-> (out_lens: list[int], digests: list[bytes], kernel_ms: float).  Refuses a ticket submitted with F_PASSTHROUGH
+        (SKY_E_INVALID), which stays waitable for wait_ex."""
+        out_lens, digests, _, _, ms = self._wait(ticket, False)
+        return out_lens, digests, ms
 
     def wait_ex(self, ticket: int):
         """Completes any ticket, and the only wait for one submitted with F_PASSTHROUGH -> (out_lens, digests, verify,
         compressed, kernel_ms).  compressed[i]: True when chunk i's payload is its frame (or the box of its frame), False when
         it is the chunk (out_len 0 without F_E2EE: the caller holds the bytes) or the box of the chunk.  verify is None unless
-        the ticket has F_VERIFY."""
+        the ticket has F_VERIFY; verify[i] is then 0 or the D_* code of chunk i's frame as the compressor made it (its payload
+        is the stored-block frame)."""
+        out_lens, digests, ver, comp, ms = self._wait(ticket, True)
+        return out_lens, digests, None if ver is None else list(ver), [bool(c) for c in comp], ms
+
+    def _wait(self, ticket: int, ex: bool):
+        """sky_wait with out_len and md5, and with verify (when the ticket has F_VERIFY) and compressed when `ex`."""
         n, _keep, flags = self._inflight[ticket]
         out = (ctypes.c_uint64 * n)()
         md5 = (ctypes.c_ubyte * (16 * n))()
-        comp = (ctypes.c_uint8 * n)()
+        ver = (ctypes.c_int32 * n)() if ex and flags & F_VERIFY else None
+        comp = (ctypes.c_uint8 * n)() if ex else None
         ms = ctypes.c_float(0)
-        has_verify = bool(flags & F_VERIFY)
-        ver = (ctypes.c_int32 * n)() if has_verify else None
-        self._check(lib().sky_wait_ex(self._h, ticket, out, md5, ver, comp, ctypes.byref(ms)))
+        self._check(lib().sky_wait(self._h, ticket, out, md5, ver, comp, ctypes.byref(ms)))
         del self._inflight[ticket]
-        raw = bytes(md5)
-        return list(out), [raw[16 * i : 16 * i + 16] for i in range(n)], list(ver) if has_verify else None, [bool(c) for c in comp], ms.value
+        return list(out), _digests(bytes(md5)), ver, comp, ms.value
 
     # ------------------------------------------------------------------ device-resident path
     def process_device(self, d_src: int, src_off: Sequence[int], src_len: Sequence[int], d_dst: int, dst_off: Sequence[int],
@@ -442,12 +425,11 @@ class Context:
         were made with; content_xxh: the chunks' XXH32, exactly when flags has F_CHECKSUM.  frame_cap None: check only;
         otherwise failing frames are rewritten as stored-block frames.  -> (status, frame_len, kernel_ms)."""
         n = len(src_len)
-        U = ctypes.c_uint64 * n
-        fl = U(*frame_len)
+        fl = _u64_array(frame_len, n)
         st = (ctypes.c_int32 * n)()
         ms = ctypes.c_float(0)
-        self._check(lib().sky_verify_device(self._h, n, d_src, U(*src_off), U(*src_len), d_frames, U(*frame_off), fl,
-                                            U(*frame_cap) if frame_cap is not None else None,
+        self._check(lib().sky_verify_device(self._h, n, d_src, _u64_array(src_off, n), _u64_array(src_len, n), d_frames,
+                                            _u64_array(frame_off, n), fl, _u64_array(frame_cap, n) if frame_cap is not None else None,
                                             (ctypes.c_uint32 * n)(*content_xxh) if content_xxh is not None else None, flags,
                                             stream or None, st, ctypes.byref(ms)))
         return list(st), list(fl), ms.value
@@ -457,14 +439,12 @@ class Context:
                       raw_len: Sequence[int], stream: int = 0):
         """-> (status: list[int], digests: list[bytes], kernel_ms)."""
         n = len(frame_len)
-        U = ctypes.c_uint64 * n
         st = (ctypes.c_int32 * n)()
         md5 = (ctypes.c_ubyte * (16 * n))()
         ms = ctypes.c_float(0)
-        self._check(lib().sky_decode_device(self._h, n, d_frames, U(*frame_off), U(*frame_len), d_out, U(*out_off), U(*raw_len),
-                                            stream or None, st, md5, ctypes.byref(ms)))
-        raw = bytes(md5)
-        return list(st), [raw[16 * i : 16 * i + 16] for i in range(n)], ms.value
+        self._check(lib().sky_decode_device(self._h, n, d_frames, _u64_array(frame_off, n), _u64_array(frame_len, n), d_out,
+                                            _u64_array(out_off, n), _u64_array(raw_len, n), stream or None, st, md5, ctypes.byref(ms)))
+        return list(st), _digests(bytes(md5)), ms.value
 
     def decode(self, frame_addrs: Sequence[int], frame_lens: Sequence[int], dst_addrs: Optional[Sequence[int]], raw_lens: Sequence[int],
                flags: int = 0):
@@ -480,8 +460,7 @@ class Context:
         ms = ctypes.c_float(0)
         self._check(lib().sky_decode(self._h, n, A(*frame_addrs), U(*frame_lens), A(*dst_addrs) if dst_addrs is not None else None,
                                      U(*raw_lens), flags, st, md5, ctypes.byref(ms)))
-        raw = bytes(md5)
-        return list(st), [raw[16 * i : 16 * i + 16] for i in range(n)], ms.value
+        return list(st), _digests(bytes(md5)), ms.value
 
     # ------------------------------------------------------------------ torch-free device memory
     def device_alloc(self, nbytes: int) -> int:

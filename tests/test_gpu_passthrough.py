@@ -133,28 +133,45 @@ class Batch:
         self.dst.close()
 
 
+def sky_wait(ctx, t, n, verify, compressed):
+    """sky_wait on ticket t with out_len and md5, and with verify[] / compressed[] when asked -> (rc, out_lens, digests,
+    verify, compressed), None for an output not asked for."""
+    out, md5 = (ctypes.c_uint64 * n)(), (ctypes.c_ubyte * (16 * n))()
+    ver = (ctypes.c_int32 * n)() if verify else None
+    comp = (ctypes.c_uint8 * n)() if compressed else None
+    rc = native.lib().sky_wait(ctx._h, t, out, md5, ver, comp, None)
+    return (rc, list(out), [bytes(md5[16 * i : 16 * i + 16]) for i in range(n)], None if ver is None else list(ver),
+            None if comp is None else [bool(c) for c in comp])
+
+
 def run(ctx, datas, flags, nonces=None):
-    """-> (out_lens, digests, verify, compressed, payloads, guards intact) of one batch; a F_PASSTHROUGH ticket must be
-    refused by sky_wait and sky_wait_verify first, and stay waitable."""
-    b = Batch(datas, flags)
-    try:
-        t = b.submit(ctx, flags, nonces)
-        if flags & native.F_PASSTHROUGH:
-            n = len(datas)
-            L = native.lib()
-            out, md5, ver = (ctypes.c_uint64 * n)(), (ctypes.c_ubyte * (16 * n))(), (ctypes.c_int32 * n)()
-            assert L.sky_wait(ctx._h, t, out, md5, None) == native.SKY_E_INVALID
-            assert L.sky_wait_verify(ctx._h, t, out, md5, ver if flags & native.F_VERIFY else None, None) == native.SKY_E_INVALID
-            assert L.sky_wait_ex(ctx._h, t, out, md5, None, None, None) == native.SKY_E_INVALID  # compressed[] is required
-            lens, dg, verify, comp, _ = ctx.wait_ex(t)
-        else:
-            lens, dg, verify, _ = ctx.wait_verify(t) if flags & native.F_VERIFY else (*ctx.wait(t)[:2], None, 0)
-            comp = [True] * len(datas)
-        payloads = [b.payload(i, n) for i, n in enumerate(lens)]
-        guards = all(b.untouched(i, n) for i, n in enumerate(lens))
-        return lens, dg, verify, comp, payloads, guards
-    finally:
-        b.close()
+    """-> (out_lens, digests, verify, compressed, payloads, guards intact) of one batch.  The batch is submitted once for
+    each (verify, compressed) request sky_wait accepts for its ticket, and every one must complete it with the same
+    results; without F_PASSTHROUGH compressed[i] is 1 exactly when the ticket has F_LZ4.  Before that, the requests the
+    ticket refuses -- verify without F_VERIFY, no compressed with F_PASSTHROUGH -- must return SKY_E_INVALID and leave it
+    waitable."""
+    n = len(datas)
+    forms = [(v, c) for v in (False, True) for c in (False, True)]
+    allowed = [(v, c) for v, c in forms if (not v or flags & native.F_VERIFY) and (c or not flags & native.F_PASSTHROUGH)]
+    got = []
+    for form in allowed:
+        b = Batch(datas, flags)
+        try:
+            t = b.submit(ctx, flags, nonces)
+            for refused in (f for f in forms if f not in allowed):
+                assert sky_wait(ctx, t, n, *refused)[0] == native.SKY_E_INVALID, refused
+            rc, lens, dg, ver, comp = sky_wait(ctx, t, n, *form)
+            assert rc == native.SKY_OK, form
+            del ctx._inflight[t]
+            got.append((lens, dg, ver, comp, [b.payload(i, k) for i, k in enumerate(lens)], all(b.untouched(i, k) for i, k in enumerate(lens))))
+        finally:
+            b.close()
+    lens, dg, _, _, payloads, guards = got[0]
+    ver = next((g[2] for g in got if g[2] is not None), None)
+    comp = next(g[3] for g in got if g[3] is not None)
+    assert all((g[0], g[1], g[4], g[5]) == (lens, dg, payloads, guards) and g[2] in (None, ver) and g[3] in (None, comp) for g in got)
+    assert flags & native.F_PASSTHROUGH or comp == [bool(flags & native.F_LZ4)] * n
+    return lens, dg, ver, comp, payloads, guards
 
 
 @pytest.mark.parametrize("verify", [False, True], ids=["noverify", "verify"])
@@ -230,7 +247,7 @@ def test_refusals_and_wait_ex_on_other_tickets(ctx):
         finally:
             ctx.device_free(d_in)
             ctx.device_free(d_out)
-        # sky_wait_ex completes any ticket: compressed[i] is 1 exactly when the ticket makes frames
+        # wait_ex completes any ticket: compressed[i] is 1 exactly when the ticket makes frames
         for flags, want in ((0, True), (native.F_LZ4 | native.F_MD5, True), (native.F_MD5, False)):
             lens_, dg, ver, comp, _ = ctx.wait_ex(b.submit(ctx, flags))
             assert comp == [want] * n and ver is None and dg == [hashlib.md5(d).digest() for d in datas]

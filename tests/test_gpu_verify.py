@@ -245,13 +245,11 @@ def test_flag_rules(ctx):
         slot = s.begin()
         s.add_bytes(slot, b"q" * 5000)
         s.launch(slot)  # without the flag: no statuses to ask for, and the ticket stays valid
-        with pytest.raises(native.SkyChunkError) as e:
-            s.ctx.wait_verify(slot.ticket)
-        assert e.value.code == native.SKY_E_INVALID
+        assert native.lib().sky_wait(s.ctx._h, slot.ticket, None, None, (ctypes.c_int32 * 1)(), None, None) == native.SKY_E_INVALID
         (r,) = s.collect(slot)
         assert r.verify_status == 0 and ref.lz4f_decompress(bytes(r.frame), 5000) == b"q" * 5000
         t = s.ctx.submit([buf.addr], [100], [buf.addr + 4096], [native.frame_need(100)], V)  # alone: LZ4 + MD5 + verify
-        lens, _, ver, _ = s.ctx.wait_verify(t)
+        lens, _, ver, _, _ = s.ctx.wait_ex(t)
         assert ver == [0] and lens[0] > 0
         buf.close()
     finally:

@@ -181,10 +181,10 @@ def test_operator_worker_loop_conventions(tmp_path):
 
 
 # ------------------------------------------------------------------ C ABI surface
-def test_abi3_header_and_library_symbols_agree():
+def test_abi4_header_and_library_symbols_agree():
     hdr = (ROOT / "include" / "skychunk.h").read_text()
     declared = set(re.findall(r"SKY_API[^;]*?\b(sky_[a-z0-9_]+)\s*\(", hdr))
-    assert declared == set(native.ABI_SYMBOLS)
+    assert declared == set(native.ABI_SYMBOLS) and len(declared) == len(native.ABI_SYMBOLS) == 24
     lib = native.lib()  # builds with nvcc if missing (cross-compiles without a GPU)
     for name in native.ABI_SYMBOLS:
         assert hasattr(lib, name), name
@@ -192,7 +192,7 @@ def test_abi3_header_and_library_symbols_agree():
     exported = set(re.findall(r" T (sky_[a-z0-9_]+)", out))
     assert exported == declared
     m = re.search(r"#define SKY_ABI_VERSION (\d+)", hdr)
-    assert lib.sky_abi_version() == int(m.group(1)) == 3
+    assert lib.sky_abi_version() == int(m.group(1)) == 4
 
 
 def test_frame_bound_and_strerror_without_gpu():
